@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/s of the batched HighwayEnv hot path on B200, every BASELINE.json config in one line.
+"""bench.py — env-steps/s of the batched HighwayEnv hot path on H100, every BASELINE.json config in one line.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
                     [--envs-per-gpu E] [--configs cfg2,cfg3] [--gather-obs] [--no-cpu-baseline]
+                    [--dump-outputs DIR]
 
 Headline (top-level keys of the JSON line) = BASELINE.json configs[1]: highway-fast-v0, vehicles_count=50
 (V = 51), 3 lanes, 5 substeps per step, Kinematics observation, DiscreteMetaAction, 4096 envs per GPU
@@ -12,22 +13,26 @@ Multi-GPU: one process per GPU (torchrun), each rank owns a contiguous env-index
 data path (weak scaling).  At N > 1 the line also carries a strong-scaling point (32 768 envs in total) and,
 with --gather-obs, the cost of the optional NCCL all-gather of the whole-batch observation.
 
-`configs` holds one entry per BASELINE.json config (cfg1..cfg5), each with
+`configs` holds one entry per BASELINE.json config (cfg1..cfg5), each timed over K steps, with
   value        device-timed throughput (CUDA events around every env.step on the launch stream, actions
                resident in HBM, L2 flushed between timed steps, max over ranks);
   e2e          the same metric through the public API with HOST buffers (pinned actions H2D, obs / reward /
                terminated / truncated D2H, sync every step; through env.host_stepper()'s CUDA graph when the
                env offers one);
-  roofline     the dominant kernel against the measured HBM peak (algorithmic bytes of SURVEY.md §8(d)), plus
-               the compute-side figures of the committed ncu capture (issue-active, fp64 pipe, thread
-               instructions per vehicle-substep) because none of these kernels is bandwidth bound;
+  roofline     the dominant kernel against the H100 SXM data-sheet HBM bandwidth (algorithmic bytes of SURVEY.md
+               §8(d)); none of these kernels is bandwidth bound;
   cpu_baseline the C oracle port of the same workload on the host cores: one pinned single-threaded process
                per core, >= 3 s timed, median of 3, load average and affinity recorded; and, quoted as
                "measured elsewhere", the per-core rate of the UNMODIFIED Python reference from
                profiles/r2_python_reference.json (tools/time_reference.py, build container).
 
---impl reference: the CPU arm of the headline config alone (the Python reference cannot travel to the GPU
-box: /root/reference is absent there and gymnasium is not installed; the C port is its line-cited restatement).
+--impl reference: the CPU arm of the headline config alone (the Python reference is not part of this repository;
+the C port is its line-cited restatement).
+
+--dump-outputs DIR: after the timed steps of every config, what the last timed env.step returned on rank 0 (obs,
+reward, terminated, truncated and the info arrays) is written as DIR/<cfg>_<name>.npy in float32 (float64 where the
+step returns float64), at most 64 MB (64·10⁶ bytes) in all (a fixed, seeded sample of env rows beyond that, listed in
+DIR/<cfg>_rows.npy).  Resets, actions and the step count are seeded, so equal arguments give equal inputs.
 """
 from __future__ import annotations
 
@@ -54,28 +59,27 @@ CONFIGS = {
         baseline="highway-fast-v0, 1 env, vehicles_count=20, Kinematics, DiscreteMetaAction (CPU plumbing case; "
                  "batched here)",
         env_id="highway-fast-v0", config=None, envs_per_gpu=4096, actions="discrete5", vehicles=21, substeps=5,
-        algo_bytes=2 * 21 * 96 + 4 + 100 + 6, kernel="highway_step_kernel<32, true>", ncu="r2_ncu_highway_step_v21.json"),
+        algo_bytes=2 * 21 * 96 + 4 + 100 + 6, kernel="highway_step_kernel<32, true>"),
     "cfg2": dict(
-        baseline="highway-fast-v0, 4096 batched envs, vehicles_count=50, Kinematics, 1xB200",
+        baseline="highway-fast-v0, 4096 batched envs, vehicles_count=50, Kinematics, 1xH100",
         env_id="highway-fast-v0", config={"vehicles_count": 50}, envs_per_gpu=4096, actions="discrete5",
-        vehicles=51, substeps=5, algo_bytes=2 * 51 * 96 + 4 + 100 + 6, kernel="highway_step_kernel<64, true>",
-        ncu="r2_ncu_highway_step_v51.json"),
+        vehicles=51, substeps=5, algo_bytes=2 * 51 * 96 + 4 + 100 + 6, kernel="highway_step_kernel<64, true>"),
     "cfg3": dict(
-        baseline="intersection-v0, 8192 envs, IDM + priority-yield, OccupancyGrid observation, 1xB200",
+        baseline="intersection-v0, 8192 envs, IDM + priority-yield, OccupancyGrid observation, 1xH100",
         env_id="intersection-v0", config={"observation": {"type": "OccupancyGrid"}}, envs_per_gpu=8192,
         actions="discrete3", vehicles=32, substeps=15, algo_bytes=2 * 32 * 128 + 4 + 1936 + 6,
-        kernel="network_step_kernel<16|32, regulated>", ncu="r2_ncu_network_step_intersection.json"),
+        kernel="network_step_kernel<16|32, regulated>"),
     "cfg4": dict(
-        baseline="roundabout-v0, 16384 envs (2 x 8192), CircularLane path, TimeToCollision observation, 2xB200",
+        baseline="roundabout-v0, 16384 envs (2 x 8192), CircularLane path, TimeToCollision observation, 2xH100",
         env_id="roundabout-v0", config={"observation": {"type": "TimeToCollision", "horizon": 10}},
         envs_per_gpu=8192, actions="discrete5", vehicles=5, substeps=15, algo_bytes=2 * 5 * 128 + 4 + 360 + 6,
-        kernel="network_step_kernel<8>", ncu="r2_ncu_network_step_roundabout.json"),
+        kernel="network_step_kernel<8>"),
     "cfg5": dict(
-        baseline="highway-v0, 65536 envs sharded 8xB200 (8192 per GPU), vehicles_count=100, Kinematics, "
+        baseline="highway-v0, 65536 envs sharded 8xH100 (8192 per GPU), vehicles_count=100, Kinematics, "
                  "ContinuousAction",
         env_id="highway-v0", config={"vehicles_count": 100, "action": {"type": "ContinuousAction"}},
         envs_per_gpu=8192, actions="box2", vehicles=101, substeps=15, algo_bytes=2 * 101 * 96 + 8 + 100 + 6,
-        kernel="highway_step_kernel<128, true>", ncu="r2_ncu_highway_step_v101.json"),
+        kernel="highway_step_kernel<128, true>"),
 }
 
 
@@ -87,7 +91,7 @@ def workload_name(key: str) -> str:
 
 # ------------------------------------------------------------------ clocks
 class ClockSampler:
-    """SM clock / throttle-reason sampling DURING the timed region (B200_PROFILING.md clocks line).
+    """SM clock / throttle-reason sampling DURING the timed region.
 
     The headline's timed region is tens of milliseconds, shorter than one `nvidia-smi -lms` period, so the samples come
     from NVML directly (the library nvidia-smi reads, via nvidia-ml-py) on a thread polling every `period` seconds; the
@@ -439,20 +443,12 @@ def run_reference_arm(args) -> None:
 
 
 # ------------------------------------------------------------------ GPU arm
-def _ncu_summary(name: str):
-    try:
-        with open(os.path.join(ROOT, "profiles", name)) as f:
-            return json.load(f)
-    except (OSError, ValueError):
-        return None
-
-
 def _peak():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (not measured)"
 
 
 def _make_actions(kind, shape_n, count, gen, dev, torch):
@@ -462,8 +458,51 @@ def _make_actions(kind, shape_n, count, gen, dev, torch):
     return torch.randint(0, hi, (count, shape_n), generator=gen, device=dev, dtype=torch.int32)
 
 
-def measure_config(key, E, K, W, rank, world, dev, ctx, do_e2e=True, gather=False):
-    """Device-timed and end-to-end throughput of one config on this rank; returns local timings."""
+def _host_outputs(out, prefix):
+    """env.step's return value as {name: host array}; the action echoed in info is an input, not an output."""
+    obs, rew, term, trunc, info = out
+    arrays = {"obs": obs, "reward": rew, "terminated": term, "truncated": trunc}
+    for k, v in info.items():
+        if isinstance(v, dict):
+            arrays.update({f"{k}_{n}": t for n, t in v.items()})
+        elif k != "action":
+            arrays[k] = v
+    return {f"{prefix}_{k}": v.detach().cpu().numpy() for k, v in arrays.items()}
+
+
+DUMP_BUDGET = 64 * 10**6  # bytes, .npy headers included
+
+
+def dump_outputs(outputs: dict, out_dir: str, budget: int = DUMP_BUDGET) -> None:
+    """Write {cfg: {name: array}} as out_dir/<name>.npy in float32 / float64 within `budget` bytes.  Configs are
+    written smallest first, each may use an equal share of what is left, so unused shares pass to the larger ones;
+    a config that still does not fit keeps a fixed, seeded sample of env rows (listed in <cfg>_rows.npy)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    header = 128  # np.save header of an array of a few dimensions
+    cast = {key: {k: v.astype(np.float64 if v.dtype == np.float64 else np.float32) for k, v in arrays.items()}
+            for key, arrays in outputs.items()}
+    size = {key: sum(v.nbytes + header for v in arrays.values()) for key, arrays in cast.items()}
+    left = budget
+    for i, key in enumerate(sorted(cast, key=lambda k: size[k])):
+        arrays, share = cast[key], left // (len(cast) - i)
+        if size[key] > share:
+            n = next(iter(arrays.values())).shape[0]
+            row_bytes = sum(v.nbytes // n for v in arrays.values()) + 8
+            m = max(0, (share - header * (len(arrays) + 1)) // row_bytes)
+            rows = np.sort(np.random.default_rng(0).choice(n, size=m, replace=False))
+            arrays = {k: v[rows] for k, v in arrays.items()}
+            arrays[f"{key}_rows"] = rows.astype(np.float64)
+        for k, v in arrays.items():
+            path = os.path.join(out_dir, k + ".npy")
+            np.save(path, np.ascontiguousarray(v))
+            left -= os.path.getsize(path)
+
+
+def measure_config(key, E, K, W, rank, world, dev, ctx, do_e2e=True, gather=False, keep_outputs=False):
+    """Device-timed and end-to-end throughput of one config on this rank; returns local timings (and, with
+    keep_outputs, what the last timed step returned, copied to the host after the timed region)."""
     import torch
     import torch.distributed as dist
 
@@ -504,17 +543,19 @@ def measure_config(key, E, K, W, rank, world, dev, ctx, do_e2e=True, gather=Fals
     for k in range(K):
         flush.fill_(k & 0xFF)  # > L2: the state is read from HBM in every timed step
         ev[k][0].record(stream)
-        env.step(actions[W + k])
+        out = env.step(actions[W + k])
         ev[k][1].record(stream)
     barrier()
     t_wall = time.perf_counter() - t_wall0
+    outputs = _host_outputs(out, key) if keep_outputs else None  # the buffers are reused by the next step
     clocks = sampler.stop() if sampler else None
     launches = int(lib.hwy_launch_count() - launches0)
     total_ms = sum(a.elapsed_time(b) for a, b in ev)
     kev, env._kernel_events = env._kernel_events, None
     kern_ms = sum(a.elapsed_time(b) for a, b in kev) / max(1, len(kev)) if kev else total_ms / K
     res = {"total_ms": total_ms, "kern_ms": kern_ms, "launches": launches, "wall_s": t_wall, "clocks": clocks,
-           "obs_bytes": int(env._obs[0].numel() * 4), "act_bytes": int(actions[0].numel() * actions.element_size() // E)}
+           "obs_bytes": int(env._obs[0].numel() * 4), "act_bytes": int(actions[0].numel() * actions.element_size() // E),
+           "outputs": outputs}
 
     if gather and world > 1:
         from highwayenv_b200.parallel import all_gather_batch
@@ -617,7 +658,7 @@ def run_gpu_arm(args) -> None:
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     K, W = args.steps, args.warmup
-    ctx = {"lib": N.load(), "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}  # > 126 MB L2
+    ctx = {"lib": N.load(), "flush": torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)}  # > 50 MB L2
     peak, peak_src = _peak()
     keys = [k for k in CONFIGS if (not args.configs or k in args.configs.split(","))]
     if HEADLINE not in keys:
@@ -642,36 +683,31 @@ def run_gpu_arm(args) -> None:
             dist.all_reduce(t)
         return int(t.item())
 
-    entries, head, head_raw = [], None, None
+    entries, head, head_raw, outputs = [], None, None, {}
     for key in keys:
         E = envs_for(key)
-        Kc = K if key == HEADLINE else max(20, min(K, args.other_steps))
-        r = measure_config(key, E, Kc, W, rank, world, dev, ctx, gather=args.gather_obs and key == HEADLINE)
+        r = measure_config(key, E, K, W, rank, world, dev, ctx, gather=args.gather_obs and key == HEADLINE,
+                           keep_outputs=bool(args.dump_outputs) and rank == 0)
+        if r["outputs"] is not None:
+            outputs[key] = r["outputs"]
         total_ms, e2e_s, e2e_eager, kern_ms = reduce_max([r["total_ms"], r["e2e_s"], r["e2e_eager_s"], r["kern_ms"]])
         launches = reduce_sum(r["launches"])
         n_total = E * world
         c = CONFIGS[key]
         achieved = c["algo_bytes"] * E / (kern_ms * 1e-3) / 1e9
-        ncu = _ncu_summary(c["ncu"]) or {}
-        traffic = (float(ncu["dram_bytes_read"]) + float(ncu["dram_bytes_write"])) if "dram_bytes_read" in ncu else None
         veh_sub = E * c["vehicles"] * c["substeps"]
         entry = {
             "id": key, "baseline_config": c["baseline"], "workload": workload_name(key),
-            "envs_per_gpu": E, "envs_total": n_total, "steps": Kc,
-            "value": n_total * Kc / (total_ms * 1e-3), "unit": UNIT, "ms_per_step": total_ms / Kc,
-            "vehicle_substeps_per_s": veh_sub * world * Kc / (total_ms * 1e-3),
+            "envs_per_gpu": E, "envs_total": n_total, "steps": K,
+            "value": n_total * K / (total_ms * 1e-3), "unit": UNIT, "ms_per_step": total_ms / K,
+            "vehicle_substeps_per_s": veh_sub * world * K / (total_ms * 1e-3),
             "gpu_launches": launches,
-            "e2e": {"value": n_total * Kc / e2e_s, "unit": UNIT, "h2d_bytes_per_step": r["h2d"],
-                    "d2h_bytes_per_step": r["d2h"], "api": r["e2e_api"], "eager_value": n_total * Kc / e2e_eager},
+            "e2e": {"value": n_total * K / e2e_s, "unit": UNIT, "h2d_bytes_per_step": r["h2d"],
+                    "d2h_bytes_per_step": r["d2h"], "api": r["e2e_api"], "eager_value": n_total * K / e2e_eager},
             "roofline": {
                 "bound": "hbm", "kernel": c["kernel"], "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": c["algo_bytes"] * E, "kernel_ms": kern_ms,
-                "issue_active_pct": ncu.get("issue_active_pct"), "fp64_pipe_pct": ncu.get("fp64_pipe_pct"),
-                "warps_active_pct": ncu.get("warps_active_pct"),
-                "thread_inst_per_vehicle_substep": ncu.get("thread_inst_per_vehicle_substep"),
-                "registers_per_thread": ncu.get("registers_per_thread"),
-                "ncu_source": ("profiles/" + c["ncu"]) if ncu else None,
                 "note": "compute/latency bound (fp64 + libm, branchy), not HBM bound: see DESIGN.md roofline",
             },
         }
@@ -690,11 +726,10 @@ def run_gpu_arm(args) -> None:
     strong = None
     if world > 1 and not args.no_strong:
         Es = STRONG_TOTAL_ENVS // world
-        r = measure_config(HEADLINE, Es, max(20, K // 2), W, rank, world, dev, ctx, do_e2e=False)
+        r = measure_config(HEADLINE, Es, K, W, rank, world, dev, ctx, do_e2e=False)
         (total_ms,) = reduce_max([r["total_ms"]])
-        Ks = max(20, K // 2)
         strong = {"scaling": "strong", "envs_total": Es * world, "envs_per_gpu": Es,
-                  "value": Es * world * Ks / (total_ms * 1e-3), "unit": UNIT, "ms_per_step": total_ms / Ks,
+                  "value": Es * world * K / (total_ms * 1e-3), "unit": UNIT, "ms_per_step": total_ms / K,
                   "note": "same total batch at every N; compare with the N=1 line run with --envs-per-gpu 32768"}
     gather = None
     if head_raw and "gather_ms" in head_raw:
@@ -704,6 +739,8 @@ def run_gpu_arm(args) -> None:
                   "algbw_GBps": head_raw["gather_bytes"] / (gms * 1e-3) / 1e9,
                   "step_ms_without": head["ms_per_step"]}
 
+    if outputs:
+        dump_outputs(outputs, args.dump_outputs)
     if rank == 0:
         if not args.no_cpu_baseline:
             for entry in entries:
@@ -746,12 +783,13 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--envs-per-gpu", type=int, default=0, help="override for the headline config")
-    ap.add_argument("--other-steps", type=int, default=50, help="timed steps of the non-headline configs")
     ap.add_argument("--configs", default="", help="comma list (cfg1..cfg5); default all")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-strong", action="store_true")
     ap.add_argument("--gather-obs", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step of every config returned as DIR/<name>.npy")
     ap.add_argument("--cpu-seconds", type=float, default=3.0)
     ap.add_argument("--cpu-repeats", type=int, default=3)
     ap.add_argument("--cpu-arm", default="", help="internal: run the CPU arm of one config and print its JSON")

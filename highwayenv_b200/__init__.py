@@ -1,4 +1,4 @@
-"""highwayenv_b200 — B200-native batched backend for HighwayEnv's simulation hot path.
+"""highwayenv_b200 — H100-native batched backend for HighwayEnv's simulation hot path.
 
 Drop-in for the path ``AbstractEnv._simulate -> Road.act / Road.step -> observe / reward``
 of Farama-Foundation/HighwayEnv 1.12.1, for thousands of independent envs at once:
@@ -9,7 +9,7 @@ of Farama-Foundation/HighwayEnv 1.12.1, for thousands of independent envs at onc
     obs, reward, terminated, truncated, info = env.step(actions)   # device tensors
 
 The env ids, ``config`` keys and observation/action plugin names are the reference's
-(highway_env/__init__.py:36-184).  Kernels are hand-written CUDA for sm_100a behind the C
+(highway_env/__init__.py:36-184).  Kernels are hand-written CUDA for sm_90a behind the C
 ABI of include/hwyb200.h; there is no CPU fallback.
 """
 from __future__ import annotations

@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/hwyb200.h.
 
 The shared library ``csrc/libhwyb200.so`` is built in-tree by ``highwayenv_b200.build``
-(nvcc, sm_100a).  There is NO CPU fallback: if the library is missing, or no CUDA device is
+(nvcc, sm_90a).  There is NO CPU fallback: if the library is missing, or no CUDA device is
 visible when a kernel entry point is called, a RuntimeError is raised.
 """
 from __future__ import annotations
@@ -229,7 +229,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -m highwayenv_b200.build` "
-            "(nvcc, sm_100a). highwayenv_b200 has no CPU fallback."
+            "(nvcc, sm_90a). highwayenv_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     lib.hwy_abi_version.restype = C.c_int

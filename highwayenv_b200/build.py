@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a kernels:  python -m highwayenv_b200.build
+"""In-tree build of the sm_90a kernels:  python -m highwayenv_b200.build
 
 nvcc cross-compiles without a GPU.  -fmad=false: the fp64 simulation follows the
 reference's separately rounded operations (explicit fma() only where numpy fuses).
@@ -16,7 +16,7 @@ DEPS = SRC + [os.path.join(_HERE, "csrc", h) for h in ("hwy_math.cuh", "hwy_devi
 OUT = os.path.join(_HERE, "csrc", "libhwyb200.so")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-fmad=false", "-Xcompiler", "-fPIC", "-shared", "--threads", "3",  # the three sources compile concurrently
 ]
 

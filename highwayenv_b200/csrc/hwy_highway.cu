@@ -1,4 +1,4 @@
-// hwy_highway.cu — sm_100a kernels + C ABI for the straight-highway family
+// hwy_highway.cu — sm_90a kernels + C ABI for the straight-highway family
 // (highway-v0 / highway-fast-v0) of the batched HighwayEnv hot path.
 //
 // Thread mapping: one (env, vehicle) pair per thread, TPE threads per env (32/64/128, the
@@ -88,9 +88,7 @@ struct EnvShared {
 
 // All envs of a block advance in lock-step (block-wide barriers): besides ordering the shared
 // staging it keeps the block's warps on the same code at the same time, which is what the
-// instruction cache wants from a ~100 KB kernel (measured: 1.4x over per-env barriers).
-// (Per-env named barriers — all of them, only the ones inside a substep, only the two around the MOBIL items — were
-// measured again on the 32 KB loop: 10.7-11.6 M against 12.8 M env-steps/s on the headline, profiles/r2_kernel_history.md.)
+// instruction cache wants from a ~100 KB kernel (per-env barriers were slower).
 template <int TPE>
 __device__ __forceinline__ void env_sync() {
     __syncthreads();
@@ -611,7 +609,7 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     if (reuse) {
         rank = active ? prev->rank[i] : 0;
     } else {
-        // (the repair pays for itself only where the count is long: V = 101 +3 %, V = 51 +-0, V = 21 -5 %)
+        // (the repair pays for itself only where the count is long, so only the 128-slot kernel uses it)
         int rt = (TPE >= 128 && prev) ? rank_repair(F, *prev, V, i, active) : -1;
         if (rt < 0) rt = rank_count(F, V, i, active);  // first frame of a launch, ties, or more than isolated swaps
         rank = rt & 0xff;
@@ -973,8 +971,8 @@ constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full regis
 // AL (host-checked, lanes_congruent): every lane is a copy of lane 0 shifted sideways — what
 // RoadNetwork.straight_road_network builds (road/road.py:291-321) — so the general-geometry branches (per-lane
 // projections in lane_distance / closest_lane, F.slow for unaligned lanes) are compiled out.  The per-substep loop
-// of this kernel is larger than the 32 KB L1.5 instruction cache and instruction fetch is one of its top stalls:
-// code bytes on the hot path are a first-order cost (profiles/r2_kernel_history.md).
+// of this kernel is about as large as the SM's instruction cache, so code bytes on the hot path are a first-order
+// cost.
 template <int TPE, bool AL>
 __global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
 highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
@@ -1588,10 +1586,9 @@ int step_envs_per_block(int tpe, int n_envs) {
         int v = atoi(e);
         if (v >= 1 && v <= max_epb) return v;
     }
-    // Two resident blocks per SM measured best (0.40 ms vs 0.43 ms for one 8-env block and
-    // 0.55 ms for eight 1-env blocks at 4096 envs x 51 vehicles): the blocks cover each other's
+    // Two resident blocks per SM (rather than one block of max_epb envs or many 1-env blocks): the blocks cover each other's
     // barrier stalls.  Small batches shrink the block so every SM still gets work.
-    int n_sm = 148;
+    int n_sm = 132;
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     int epb = max_epb >= 2 ? max_epb / 2 : 1;

@@ -1,4 +1,4 @@
-// hwy_math.cuh — scalar helpers shared by the sm_100a kernels.
+// hwy_math.cuh — scalar helpers shared by the sm_90a kernels.
 //
 // The simulation arithmetic is fp64 and follows the reference's operation order; the
 // translation unit is compiled with -fmad=false so the compiler never contracts a*b+c.
@@ -51,8 +51,8 @@ static __device__ __noinline__ double m_sin(double x) { return sin(x); }
 // sin and cos together.  Headings and lane phases are almost always within +-pi/4 (a vehicle following its lane),
 // where no argument reduction is needed: the fdlibm kernel polynomials (__kernel_sin / __kernel_cos, < 1 ulp, the
 // same accuracy class as numpy's and CUDA's own routines) cost ~30 fp64 operations instead of the ~300 issued
-// instructions of the general sincos(), which had become the largest single item of the step kernel (14 % of its
-// instructions, profiles/r1_step_kernel_history.md).  Larger arguments take the library routine.  Returned by
+// instructions of the general sincos(), which had become the largest single item of the step kernel's
+// instructions.  Larger arguments take the library routine.  Returned by
 // value: pointer results through a non-inlined call would live in local memory.
 static __device__ __noinline__ double2 m_sincos_impl(double x) {
     const double ax = fabs(x);
@@ -105,8 +105,7 @@ __device__ __forceinline__ double div_finite(double n, double d) { return n == 0
 // exp(y log x) — the error of log(x) is multiplied by y log x — is small here because |d log x| <= 0.35 for x in
 // [0.5, 2] (ratios of a speed to its target): ~1.5 ulp on top of the two functions' own 1 ulp, the same class as the
 // library pow's 2 ulp bound, and an absolute error below 1e-15 * x^delta for small x where (1 - x^delta) is what is
-// used.  It replaces ~175 issued instructions per call (7 % of the highway step kernel's instructions,
-// profiles/r2_kernel_history.md) by ~80.  HWY_LIBRARY_POW restores the library call.
+// used.  It replaces ~175 issued instructions per call by ~80.  HWY_LIBRARY_POW restores the library call.
 static __device__ __noinline__ double m_exp_dlog(double d, double x) { return exp(d * log(x)); }
 __device__ __forceinline__ double idm_pow(double x, double delta) {
 #ifndef HWY_LIBRARY_POW

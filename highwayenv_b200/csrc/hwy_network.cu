@@ -1,4 +1,4 @@
-// hwy_network.cu — sm_100a kernels + C ABI for envs on a GENERAL road network: roundabout-v0|v1, merge-v0|v1,
+// hwy_network.cu — sm_90a kernels + C ABI for envs on a GENERAL road network: roundabout-v0|v1, merge-v0|v1,
 // two-way-v0, u-turn-v0|v1 (8 vehicle slots per env) and intersection-v0|v2, intersection-multi-agent-v0|v1|v2
 // (16 / 32 slots, RegulatedRoad, a population that changes every step).
 // StraightLane / SineLane / CircularLane geometry, planned routes with RoadNetwork.next_lane, IDM + MOBIL with the
@@ -36,8 +36,8 @@ using namespace hwy;
 constexpr int R = HWY_NET_MAX_ROUTE;
 constexpr int kBlockThreads = 256;  // observe / substeps / debug kernels
 // The step kernels run ONE block per SM (128 registers x 512 threads): one instruction stream per SM.  The step body is
-// ~110 KB of SASS against a 32 KB instruction cache, and two co-resident blocks in different phases evict each other:
-// 512 x 1 measured +12-14 % over 256 x 2 (same warps per SM), 128 x 4 -20 % (profiles/r2_kernel_history.md).  The
+// ~110 KB of SASS against a much smaller instruction cache, and two co-resident blocks in different phases evict each
+// other: 512 x 1 was faster than 256 x 2 (same warps per SM) and 128 x 4.  The
 // launch uses fewer threads per block when that spreads the envs over all SMs (step_plan).
 #ifndef HWY_NET_STEP_THREADS
 #define HWY_NET_STEP_THREADS 512
@@ -430,8 +430,7 @@ __device__ __forceinline__ void closest_lane_group(const GraphShared& g, EnvStag
     }
     // (this barrier and the one that ends the function are not needed for memory ordering — n_cand could be re-armed in
     // the reduce phase and nothing after the function reads another vehicle's lane before the next barrier — but removing
-    // them cost 10-25 %: the block-wide barriers keep the block's warps on the same instruction-cache lines, measured
-    // again in round 2, profiles/r2_kernel_history.md)
+    // them was slower: the block-wide barriers keep the block's warps on the same instruction-cache lines)
     phase_sync<G>();
     if (active) {
         const int hint = bl;
@@ -928,7 +927,7 @@ __device__ __forceinline__ bool corner_inside(double c1x, double c1y, double s1,
 }
 // Both directions for two rectangles of the same size.  Inlined into enforce_road_rules, which is itself a real call
 // from the substep loop (enforce_road_rules_call): its two unrolled copies used to be 13 KB in the middle of that
-// loop.  Measured on cfg 3 (profiles/r2_kernel_history.md): rolled loops -7 %, a call per pair -4 %, this form +5 %.
+// loop; rolled loops and a call per pair were both slower on cfg 3 than this form.
 __device__ __forceinline__ bool rotated_rectangles_intersect(double c1x, double c1y, double a1, double c2x, double c2y,
                                                           double a2, double l, double w) {
     double s1, c1, s2, c2;
@@ -965,7 +964,7 @@ __device__ __forceinline__ bool has_corner_inside(double c1x, double c1y, double
 // regulation.py:42-111: enforce_road_rules with is_conflict_possible / respect_priorities.
 // All threads of the group call this; r is the caller's vehicle.
 // PLAIN: the env may hold a ContinuousAction ego (kind HWY_KIND_VEHICLE); compiled out otherwise so that the
-// DiscreteMetaAction kernels keep their register budget (198 vs 128 registers measured with the code always in)
+// DiscreteMetaAction kernels keep their register budget
 template <int G, bool REG, bool PLAIN>
 __device__ __forceinline__ void enforce_road_rules(const bool dynamical, const GraphShared& g,
                                                    EnvStage<G, REG>& st, int V, int i, Regs& r, double act_steer) {
@@ -2054,8 +2053,8 @@ intersection_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGr
 // on the env's numpy stream: every lane of the warp walks it redundantly (same instructions, same values — no
 // shuffles), and the expensive part, RoadObject.__init__'s closest-lane search over all 32 lanes of the network for
 // each of the 5 vehicles (objects.py:46-50), is spread over the warp: lane l evaluates graph lane l, then a
-// (distance, index) minimum over the warp = np.argmin's first minimum.  One thread per env spent 165 us per step on
-// the ~9 % of the envs that had ended (16 % of a cfg 4 step).
+// (distance, index) minimum over the warp = np.argmin's first minimum (one thread per env made the reset a large share
+// of a cfg 4 step).
 __global__ void __launch_bounds__(128)
 roundabout_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyRoundaboutSpawn SP,
                         const __grid_constant__ HwyNetState S, uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a,
@@ -2502,8 +2501,8 @@ int blocks_for(int n_envs, int g) {
 }
 
 // Block shape of a step launch: the fewest whole waves of one block per SM that cover n_envs, the envs spread evenly
-// over waves x SMs blocks (8 192 roundabout envs, 8 slots: 147 blocks of 56 envs = 448 threads instead of 128 blocks
-// of 64 envs on 148 SMs).  Work-list launches (16- / 32-slot intersection kernels) are planned for n_envs, the upper
+// over waves x SMs blocks (6 336 roundabout envs, 8 slots, 132 SMs: 132 blocks of 48 envs = 384 threads instead of 99
+// blocks of 64 envs).  Work-list launches (16- / 32-slot intersection kernels) are planned for n_envs, the upper
 // bound of a list known only on the device; blocks past the list's end leave at once.
 struct StepPlan {
     int threads, blocks, per;
@@ -2512,10 +2511,10 @@ struct StepPlan {
 int sm_count() {
     static std::atomic<int> cached[64];
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     int n = cached[dev].load(std::memory_order_relaxed);
     if (n == 0) {
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev].store(n, std::memory_order_relaxed);
     }
     return n;

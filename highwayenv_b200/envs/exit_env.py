@@ -1,4 +1,4 @@
-"""Batched exit-v0 / exit-v1 on the B200 backend.
+"""Batched exit-v0 / exit-v1 on the H100 backend.
 
 Host-side mirror of the reference's ``ExitEnv`` (highway_env/envs/exit_env.py:15-210): a highway in three sections
 ("0"->"1" with `lanes_count` lanes, "1"->"2" with one more — the exit lane —, "2"->"3") and a circular exit ramp

@@ -1,4 +1,4 @@
-"""Batched highway-v0 / highway-fast-v0 on the B200 backend.
+"""Batched highway-v0 / highway-fast-v0 on the H100 backend.
 
 Host-side mirror of the reference's ``HighwayEnv`` / ``HighwayEnvFast``
 (highway_env/envs/highway_env.py:16-182) over ``AbstractEnv``
@@ -44,7 +44,7 @@ def _pcg64_words(seeds: Sequence[int]) -> np.ndarray:
 
 
 class BatchedHighwayEnv(ObservationHost):
-    """``num_envs`` independent highway roads stepped by the sm_100a kernels."""
+    """``num_envs`` independent highway roads stepped by the sm_90a kernels."""
 
     ENV_ID = "highway-v0"
     OTHERS_CHECK_COLLISIONS = True
@@ -64,7 +64,7 @@ class BatchedHighwayEnv(ObservationHost):
         if render_mode is not None:
             raise NotImplementedError("rendering is out of scope of the accelerated path (render_mode=None)")
         if not torch.cuda.is_available():
-            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self._lib = N.load()
         self.render_mode = None
         self.num_envs = int(num_envs)

@@ -1,4 +1,4 @@
-"""Batched intersection-v0 on the B200 backend.
+"""Batched intersection-v0 on the H100 backend.
 
 Host-side mirror of the reference's ``IntersectionEnv`` (highway_env/envs/intersection_env.py):
 4-way crossing with 20 lanes and priorities, ``RegulatedRoad`` yielding rules, a population that
@@ -90,7 +90,7 @@ class BatchedIntersectionEnv(ObservationHost):
         if render_mode is not None:
             raise NotImplementedError("rendering is out of scope of the accelerated path")
         if not torch.cuda.is_available():
-            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if autoreset_mode not in ("SameStep", "NextStep", "Disabled"):
             raise ValueError(autoreset_mode)
         if autoreset_mode == "NextStep" and reset_mode != "device":

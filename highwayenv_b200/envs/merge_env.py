@@ -1,4 +1,4 @@
-"""Batched merge-v0 / merge-v1 on the B200 backend.
+"""Batched merge-v0 / merge-v1 on the H100 backend.
 
 Host-side mirror of the reference's ``MergeEnv`` (highway_env/envs/merge_env.py): a two-lane highway a->b->c->d
 with an access ramp j->k (straight) ->b (sine) ->c (third, forbidden lane) that ends on an ``Obstacle``; the

@@ -1,4 +1,4 @@
-"""Batched roundabout-v0 on the B200 backend.
+"""Batched roundabout-v0 on the H100 backend.
 
 Host-side mirror of the reference's ``RoundaboutEnv`` (highway_env/envs/roundabout_env.py:12-391):
 same config dictionary, road geometry and spawn procedure; stepping runs in
@@ -168,7 +168,7 @@ class BatchedRoundaboutEnv(ObservationHost):
         if render_mode is not None:
             raise NotImplementedError("rendering is out of scope of the accelerated path")
         if not torch.cuda.is_available():
-            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("highwayenv_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         if autoreset_mode not in ("SameStep", "NextStep", "Disabled"):
             raise ValueError(autoreset_mode)
         if autoreset_mode == "NextStep" and reset_mode != "device":

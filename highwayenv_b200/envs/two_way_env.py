@@ -1,4 +1,4 @@
-"""Batched two-way-v0 on the B200 backend.
+"""Batched two-way-v0 on the H100 backend.
 
 Host-side mirror of the reference's ``TwoWayEnv`` (highway_env/envs/two_way_env.py): a two-lane road a->b whose left
 lane is shared with oncoming traffic on ("b", "a", 0); the controlled MDPVehicle, three IDM vehicles ahead and two

@@ -1,4 +1,4 @@
-"""Batched u-turn-v0 on the B200 backend.
+"""Batched u-turn-v0 on the H100 backend.
 
 Host-side mirror of the reference's ``UTurnEnv`` (highway_env/envs/u_turn_env.py): two lanes a->b, a
 counter-clockwise circular U-turn b->c (two CircularLanes), two lanes c->d back; the controlled MDPVehicle and six

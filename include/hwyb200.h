@@ -1,5 +1,5 @@
 /*
- * hwyb200.h — C ABI of the B200-native batched HighwayEnv hot path.
+ * hwyb200.h — C ABI of the H100-native batched HighwayEnv hot path.
  *
  * Plain pointers and sizes only (no torch / C++ types).  Every pointer in the *State
  * structs and every array argument is a DEVICE pointer owned by the caller (the Python

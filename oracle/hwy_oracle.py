@@ -8,6 +8,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import warnings
 
 import numpy as np
 
@@ -107,15 +108,15 @@ class OrcBatch(C.Structure):
     )
 
 
+def _stale() -> bool:
+    src = [os.path.join(_HERE, f) for f in ("hwy_oracle.c", "hwy_oracle.h")]
+    return not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(map(os.path.getmtime, src))
+
+
 def build(force: bool = False) -> str:
     """Compile the oracle with gcc (seconds).  Building the checker is not using it."""
     src = os.path.join(_HERE, "hwy_oracle.c")
-    hdr = os.path.join(_HERE, "hwy_oracle.h")
-    if (
-        force
-        or not os.path.exists(_LIB_PATH)
-        or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(src), os.path.getmtime(hdr))
-    ):
+    if force or _stale():
         subprocess.check_call(
             [
                 "gcc", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-std=gnu11",
@@ -131,7 +132,10 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
+        if not os.path.exists(_LIB_PATH):  # build() made it; a read-only tree must not be written to
+            build()
+        elif _stale():
+            warnings.warn(f"{_LIB_PATH} is older than its sources: run build() to use the edited oracle")
         _lib = C.CDLL(_LIB_PATH)
         _lib.orc_wrap_to_pi.restype = C.c_double
         _lib.orc_wrap_to_pi.argtypes = [C.c_double]

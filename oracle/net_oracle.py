@@ -5,6 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+import warnings
 
 import numpy as np
 
@@ -117,10 +118,14 @@ class NetState(C.Structure):
                    ("yaw_rate", C.c_void_p)])
 
 
+def _stale() -> bool:
+    src = [os.path.join(_HERE, f) for f in ("net_oracle.c", "net_oracle.h")]
+    return not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(map(os.path.getmtime, src))
+
+
 def build(force: bool = False) -> str:
-    src, hdr = os.path.join(_HERE, "net_oracle.c"), os.path.join(_HERE, "net_oracle.h")
-    if force or not os.path.exists(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(
-            os.path.getmtime(src), os.path.getmtime(hdr)):
+    src = os.path.join(_HERE, "net_oracle.c")
+    if force or _stale():
         subprocess.check_call(["gcc", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-std=gnu11",
                                "-o", _LIB_PATH, src, "-lm"])
     return _LIB_PATH
@@ -132,7 +137,10 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        build()
+        if not os.path.exists(_LIB_PATH):  # build() made it; a read-only tree must not be written to
+            build()
+        elif _stale():
+            warnings.warn(f"{_LIB_PATH} is older than its sources: run build() to use the edited oracle")
         _lib = C.CDLL(_LIB_PATH)
         _lib.net_step.restype = None
         _lib.net_step.argtypes = [C.POINTER(NetGraph), C.POINTER(NetCfg), C.POINTER(NetState), C.c_int,

@@ -20,6 +20,16 @@ def load_golden(name: str) -> dict:
     return d
 
 
+def load_pinned(path: str):
+    """A tests/golden/pinned_*.npz case of oracle/gen_pinned.py: (config, [state after t steps], other arrays)."""
+    z = np.load(path, allow_pickle=False)
+    d = {k: z[k] for k in z.files}
+    cfg = json.loads(str(d.pop("config_json")))
+    keys = [k for k in d if k.startswith("s_")]
+    states = [{k[2:]: d[k][t] for k in keys} for t in range(d[keys[0]].shape[0])]
+    return cfg, states, {k: v for k, v in d.items() if not k.startswith("s_")}
+
+
 def golden_state(g: dict, i: int, t: int) -> dict:
     """State of seed-slot i after t steps, in ref_harness.dump_state layout."""
     keys = ("x", "y", "heading", "speed", "target_speed", "timer", "delta", "lane", "target_lane",

@@ -1,5 +1,5 @@
 """The per-substep loop of the highway step kernel has to stay near the 32 KB L1.5 instruction cache: cutting it from
-70 KB to 32 KB was worth +9 % on the headline config (profiles/r2_kernel_history.md), and a stray inlined helper or
+70 KB to 32 KB made the headline config faster, and a stray inlined helper or
 unrolled loop silently undoes that.  Cross-compiles hwy_highway.cu (no GPU needed) and measures the loop statically
 with tools/loop_size.sh."""
 import ast

@@ -1,65 +1,30 @@
-"""Network oracle vs the LIVE reference on seeds that are not in the golden fixtures (only where /root/reference
-is mounted: the build container; skipped on the GPU box).  Teacher-forced, one env at a time.  intersection ids are
-left to the fixtures: IntersectionEnv._make_vehicles rewrites IDMVehicle class constants for the whole process."""
+"""Network oracle vs the reference on seeds that are not in the 32-seed fixtures, teacher-forced, one env at a time.
+The reference's states, rewards, flags and observations are stored in tests/golden/pinned_network_*.npz
+(oracle/gen_pinned.py).  intersection ids: tests/test_intersection_oracle_live.py."""
 import numpy as np
 import pytest
 
 import net_oracle as no
-import ref_harness as rh
-from parity_utils import compare_state
-
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="reference not mounted")
+from gen_pinned import NETWORK, case_path
+from parity_utils import compare_state, load_pinned
 
 
-def _state(env, V):
-    st = rh.dump_state(env)
-    st["target_lane"] = np.where(st["target_lane"] < 0, st["lane"], st["target_lane"])
-    if "route" not in st:
-        st["route"], st["route_len"] = np.zeros((V, no.NET_MAX_ROUTE), dtype=np.int32), np.zeros(V, dtype=np.int32)
-    if "kind" in st:
-        st["impact"] = np.where((st["kind"] == 3)[:, None], np.nan, st["impact"])  # objects: inert zeros
-    else:
-        st["kind"] = np.array([1] + [0] * (V - 1), dtype=np.int32)
-    st.setdefault("count", V)
-    st.setdefault("is_yielding", np.zeros(V, dtype=np.int32))
-    st.setdefault("road_steps", 0)
-    return st
-
-
-@pytest.mark.parametrize("env_id,over,T,seeds", [
-    ("roundabout-v0", {"observation": {"type": "TimeToCollision", "horizon": 10}}, 11, (31, 32)),
-    ("roundabout-v1", None, 11, (33,)),
-    ("merge-v0", None, 14, (34, 35)),
-    ("merge-v1", None, 14, (36,)),
-    ("two-way-v0", None, 10, (37, 38)),
-    ("u-turn-v0", None, 10, (39, 40)),
-    ("u-turn-v1", None, 10, (41,)),
-])
+@pytest.mark.parametrize("env_id,over,T,seeds", NETWORK)
 def test_net_oracle_matches_live_reference(env_id, over, T, seeds):
     for seed in seeds:
-        env = rh.make_reference_env(env_id, over)
-        obs_ref, _ = env.reset(seed=seed)
-        cfg = dict(env.config)
-        cfg["_env_id"] = env_id
-        if env_id.startswith("merge"):
-            lanes = [li for li, _ in rh.lane_list(env)]
-            cfg["_merge_lane"] = lanes.index(("b", "c", 2))
-            cfg["_default_side_lanes"] = len(env.road.network.all_side_lanes(env.vehicle.lane_index))
-        V = len(env.road.vehicles) + len(env.road.objects)
-        graph = no.graph_from_arrays(rh.dump_network(env))
-        oc = no.cfg_from_dict(cfg, n_vehicles=V)
-        ob = no.NetOracleBatch(graph, oc, 1)
-        ob.load_state(0, _state(env, V))
-        assert np.max(np.abs(ob.observe().reshape(np.asarray(obs_ref).shape) - obs_ref)) <= 1e-6
-        rng = np.random.default_rng(seed)
+        cfg, states, ref = load_pinned(case_path("network", env_id, seed))
+        V = int(ref["n_vehicles"])
+        ob = no.NetOracleBatch(no.graph_from_arrays(ref), no.cfg_from_dict(cfg, n_vehicles=V), 1)
+        ob.load_state(0, states[0])
+        assert np.max(np.abs(ob.observe().reshape(ref["obs"][0].shape) - ref["obs"][0])) <= 1e-6
         for t in range(T):
-            ob.load_state(0, _state(env, V))  # teacher-forced
-            a = int(rng.integers(5))
-            o, r, te, tr, _ = env.step(a)
-            oo, ro, teo, tro = ob.step([a])
+            ob.load_state(0, states[t])  # teacher-forced
+            oo, ro, teo, tro = ob.step([int(ref["actions"][t])])
             got = {k: ob.a[k][0] for k in ob.a if k not in ("speed_index", "time")}
             got["speed_index"] = ob.a["speed_index"][0]
             ctx = f"{env_id} seed {seed} t={t}"
-            assert compare_state(_state(env, V), got, ctx=ctx) < 1e-9
-            assert abs(r - ro[0]) < 1e-9 and te == bool(teo[0]) and tr == bool(tro[0]), ctx
-            assert np.max(np.abs(np.asarray(o) - oo[0].reshape(np.asarray(o).shape))) <= 1e-6, ctx
+            assert compare_state(states[t + 1], got, ctx=ctx) < 1e-9
+            assert abs(ref["reward"][t] - ro[0]) < 1e-9, ctx
+            assert bool(ref["terminated"][t]) == bool(teo[0]) and bool(ref["truncated"][t]) == bool(tro[0]), ctx
+            o = ref["obs"][t + 1]
+            assert np.max(np.abs(o - oo[0].reshape(o.shape))) <= 1e-6, ctx

@@ -1,11 +1,12 @@
-"""RoadNetwork.to_config / from_config (road/road.py:370-389; lane.py:214-233, 290-309, 360-384) on the host lane table:
-live against the mounted reference (skipped on the GPU box, where /root/reference does not exist)."""
+"""RoadNetwork.to_config / from_config (road/road.py:370-389; lane.py:214-233, 290-309, 360-384) on the host lane table,
+against the reference's own `to_config()` dicts stored in tests/golden/pinned_to_config_*.json (oracle/gen_pinned.py)."""
+import json
+import os
+
 import numpy as np
 import pytest
 
-import ref_harness as rh
-
-pytestmark = pytest.mark.skipif(not rh.reference_available(), reason="needs /root/reference (build container)")
+from gen_pinned import OUT
 
 BUILDERS = {
     "roundabout-v0": ("highwayenv_b200.envs.roundabout_env", "make_roundabout_network"),
@@ -32,24 +33,15 @@ def strip(cfg):
 
 
 @pytest.mark.parametrize("env_id", sorted(BUILDERS))
-def test_to_config_and_from_config_round_trip(env_id):
+def test_to_config_matches_reference_and_from_config_rebuilds_table(env_id):
     import importlib
 
     from highwayenv_b200.road.network import NetworkTable
 
     mod, fn = BUILDERS[env_id]
     ours = getattr(importlib.import_module(mod), fn)()
-    rh._ensure_imports()
-    from highway_env.vehicle.behavior import IDMVehicle
-
-    saved = {k: getattr(IDMVehicle, k) for k in ("DISTANCE_WANTED", "COMFORT_ACC_MAX", "COMFORT_ACC_MIN")}
-    try:  # IntersectionEnv._make_vehicles rewrites these class constants for the whole process (:262-265)
-        env = rh.make_reference_env(env_id, None)
-        env.reset(seed=0)
-        ref_cfg = env.road.network.to_config()
-    finally:
-        for k, v in saved.items():
-            setattr(IDMVehicle, k, v)
+    with open(os.path.join(OUT, "pinned_to_config_" + env_id.replace("-", "_") + ".json")) as f:
+        ref_cfg = json.load(f)
     # 1. our dict equals the reference's (insertion order included), rendering attributes aside
     a, b = strip(ours.to_config()), strip(ref_cfg)
     assert list(a) == list(b)
@@ -62,8 +54,3 @@ def test_to_config_and_from_config_round_trip(env_id):
     for k, v in ours.arrays.items():
         assert np.array_equal(back.arrays[k], v), k
     assert np.array_equal(back.succ, ours.succ) and back.index == ours.index
-    # 3. and our own dict round-trips through the reference's from_config
-    from highway_env.road.road import RoadNetwork
-
-    ref_back = RoadNetwork.from_config(ours.to_config())
-    assert strip(ref_back.to_config()) == b

@@ -5,7 +5,7 @@
 set -e
 SRC=${1:-hwy_highway.cu}; PAT=${2:-highway_step_kernelILi64ELb1}; shift 2 2>/dev/null || true
 OUT=/tmp/hwy_loop_size; mkdir -p $OUT
-nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -fmad=false -cubin "$@" \
+nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -fmad=false -cubin "$@" \
   -o $OUT/k.cubin highwayenv_b200/csrc/$SRC
 nvdisasm -g $OUT/k.cubin > $OUT/all.dis
 PAT=$PAT python - <<'P'

@@ -7,7 +7,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 label = sys.argv[1] if len(sys.argv) > 1 else os.environ.get("HWYB200_LIB", "default")
-out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--no-cpu-baseline", "--steps", "60", "--other-steps", "40"]
+out = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--no-cpu-baseline", "--steps", "40"]
                      + (["--configs", os.environ["QB_CONFIGS"]] if os.environ.get("QB_CONFIGS") else []),
                      capture_output=True, text=True)
 if out.returncode != 0:
