@@ -12,7 +12,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HWYB200_LIB") or os.path.join(_HERE, "csrc", "libhwyb200.so")
 
-HWY_ABI_VERSION = 13  # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
+HWY_ABI_VERSION = 14 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
 HWY_MAX_LANES = 8
 HWY_MAX_TARGET_SPEEDS = 8
 HWY_MAX_VEHICLES = 128
@@ -215,8 +215,16 @@ EXPORTS = (
     "hwy_network_obs_size", "hwy_network_step", "hwy_network_observe", "hwy_roundabout_reset",
     "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset", "hwy_intersection_step_agents",
     "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
-    "hwy_two_way_reset", "hwy_u_turn_reset",
+    "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64",
 )
+
+# hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
+MATH_OPS = {"sincos": (0, 1, 2), "idm_pow": (1, 2, 1), "exp_dlog": (2, 2, 1), "py_mod_pos": (3, 2, 1),
+            "wrap_to_pi": (4, 1, 1), "not_zero": (5, 1, 1), "div_finite": (6, 2, 1), "dot2": (7, 4, 1),
+            "norm2": (8, 2, 1), "beta_of_controlled": (9, 1, 2), "beta_of_angle": (10, 1, 2),
+            "speed_to_index": (11, 2 + HWY_MAX_TARGET_SPEEDS, 1)}
+# hwy_debug_pcg64 draw kinds
+PCG_OPS = {"next64": 0, "next32": 1, "next_double": 2, "uniform": 3, "normal": 4, "choice": 5, "pcg_at": 6}
 
 _lib = None
 
@@ -267,6 +275,11 @@ def load():
     lib.hwy_debug_network_neighbours.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_debug_rotated_rectangles_intersect.restype = C.c_int
     lib.hwy_debug_rotated_rectangles_intersect.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    lib.hwy_debug_math.restype = C.c_int
+    lib.hwy_debug_math.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    lib.hwy_debug_pcg64.restype = C.c_int
+    lib.hwy_debug_pcg64.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_void_p]
     lib.hwy_u_turn_reset.restype = C.c_int
     lib.hwy_u_turn_reset.argtypes = [NP, NG, C.POINTER(HwyUTurnSpawn), NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]

@@ -1511,6 +1511,100 @@ highway_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwa
     S.rng[4 * (size_t)n + e] = ((u64)g.has32 << 32) | g.u32;
 }
 
+// ------------------------------------------------------------------ test entries
+// The production device functions on one input per thread (hwy_debug_math); the operands of each HWY_MATH_* op
+// are listed in include/hwyb200.h.
+__host__ __device__ inline int math_in_width(int op) {
+    switch (op) {
+        case HWY_MATH_DOT2: return 4;
+        case HWY_MATH_SPEED_TO_INDEX: return 2 + HWY_MAX_TARGET_SPEEDS;
+        case HWY_MATH_IDM_POW: case HWY_MATH_EXP_DLOG: case HWY_MATH_PY_MOD_POS: case HWY_MATH_DIV_FINITE:
+        case HWY_MATH_NORM2: return 2;
+        default: return 1;
+    }
+}
+__host__ __device__ inline int math_out_width(int op) {
+    return op == HWY_MATH_SINCOS || op == HWY_MATH_BETA_CONTROLLED || op == HWY_MATH_BETA_ANGLE ? 2 : 1;
+}
+__global__ void debug_math_kernel(int op, const double* __restrict__ in, double* __restrict__ out, int n) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const double* a = in + (size_t)k * math_in_width(op);
+    double* o = out + (size_t)k * math_out_width(op);
+    switch (op) {
+        case HWY_MATH_SINCOS: m_sincos(a[0], &o[0], &o[1]); break;
+        case HWY_MATH_IDM_POW: o[0] = idm_pow(a[0], a[1]); break;
+        case HWY_MATH_EXP_DLOG: o[0] = m_exp_dlog(a[0], a[1]); break;
+        case HWY_MATH_PY_MOD_POS: o[0] = py_mod_pos(a[0], a[1]); break;
+        case HWY_MATH_WRAP_TO_PI: o[0] = wrap_to_pi(a[0]); break;
+        case HWY_MATH_NOT_ZERO: o[0] = not_zero(a[0]); break;
+        case HWY_MATH_DIV_FINITE: o[0] = div_finite(a[0], a[1]); break;
+        case HWY_MATH_DOT2: o[0] = dot2(a[0], a[1], a[2], a[3]); break;
+        case HWY_MATH_NORM2: o[0] = norm2(a[0], a[1]); break;
+        case HWY_MATH_BETA_CONTROLLED: beta_of_controlled(a[0], o[0], o[1]); break;
+        case HWY_MATH_BETA_ANGLE: beta_of_angle(a[0], o[0], o[1]); break;
+        case HWY_MATH_SPEED_TO_INDEX: {
+            if (!(a[1] >= 1.0 && a[1] <= (double)HWY_MAX_TARGET_SPEEDS)) {  // outside the table: no index
+                o[0] = __longlong_as_double(0x7ff8000000000000LL);
+                break;
+            }
+            HwyHighwayParams P;
+            P.n_target_speeds = (int)a[1];
+            for (int j = 0; j < HWY_MAX_TARGET_SPEEDS; ++j) P.target_speeds[j] = a[2 + j];
+            o[0] = (double)speed_to_index(P, a[0]);
+            break;
+        }
+    }
+}
+
+// count draws of one kind from the generator of each thread (words [5][n], the HwyHighwayState.rng layout);
+// draws [n][count] (doubles as their bits), for HWY_PCG_NORMAL [n][count][2] = (value bits, 64-bit outputs consumed).
+__global__ void debug_pcg64_kernel(int op, int arg_i, double arg_lo, double arg_hi, int count,
+                                   const uint64_t* __restrict__ words_in, uint64_t* __restrict__ words_out,
+                                   uint64_t* __restrict__ draws, int n) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    Pcg64 g;
+    g.s_hi = words_in[0 * (size_t)n + e];
+    g.s_lo = words_in[1 * (size_t)n + e];
+    g.i_hi = words_in[2 * (size_t)n + e];
+    g.i_lo = words_in[3 * (size_t)n + e];
+    const uint64_t w4 = words_in[4 * (size_t)n + e];
+    g.has32 = (uint32_t)(w4 >> 32);
+    g.u32 = (uint32_t)w4;
+    if (op == HWY_PCG_AT) {
+        g = pcg_at(g, arg_i);
+    } else {
+        uint64_t* d = draws + (size_t)e * count * (op == HWY_PCG_NORMAL ? 2 : 1);
+        for (int j = 0; j < count; ++j) {
+            switch (op) {
+                case HWY_PCG_NEXT64: d[j] = g.next64(); break;
+                case HWY_PCG_NEXT32: d[j] = g.next32(); break;
+                case HWY_PCG_NEXT_DOUBLE: d[j] = (uint64_t)__double_as_longlong(g.next_double()); break;
+                case HWY_PCG_UNIFORM: d[j] = (uint64_t)__double_as_longlong(g.uniform(arg_lo, arg_hi)); break;
+                case HWY_PCG_CHOICE: d[j] = (uint64_t)g.choice(arg_i); break;
+                case HWY_PCG_NORMAL: {
+                    const Pcg64 before = g;
+                    d[2 * j] = (uint64_t)__double_as_longlong(g.normal());
+                    // outputs consumed: the smallest k with before advanced by k == after (0: more than 16)
+                    uint64_t used = 0;
+                    for (int k = 1; k <= 16 && !used; ++k) {
+                        const Pcg64 a = pcg_at(before, k);
+                        if (a.s_hi == g.s_hi && a.s_lo == g.s_lo) used = k;
+                    }
+                    d[2 * j + 1] = used;
+                    break;
+                }
+            }
+        }
+    }
+    words_out[0 * (size_t)n + e] = g.s_hi;
+    words_out[1 * (size_t)n + e] = g.s_lo;
+    words_out[2 * (size_t)n + e] = g.i_hi;
+    words_out[3 * (size_t)n + e] = g.i_lo;
+    words_out[4 * (size_t)n + e] = ((uint64_t)g.has32 << 32) | g.u32;
+}
+
 }  // namespace hwy
 
 // ====================================================================== C ABI
@@ -1725,6 +1819,33 @@ int hwy_debug_phase_cycles(unsigned long long* out16) {
     for (int k = 0; k < 16; ++k) out16[k] = 0;
     return 0;
 #endif
+}
+
+int hwy_debug_math(int op, const double* in, double* out, int n, void* stream) {
+    if (op < HWY_MATH_SINCOS || op > HWY_MATH_SPEED_TO_INDEX) return fail("%s", "hwy_debug_math: unknown op");
+    if (n < 0) return fail("%s", "hwy_debug_math: n < 0");
+    if (!in || !out) return fail("%s", "hwy_debug_math: null pointer");
+    if (n == 0) return 0;
+    hwy::debug_math_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(op, in, out, n);
+    return check_launch("debug_math_kernel");
+}
+
+int hwy_debug_pcg64(int op, int arg_i, double arg_lo, double arg_hi, int count, const uint64_t* words_in,
+                    uint64_t* words_out, uint64_t* draws, int n, void* stream) {
+    if (op < HWY_PCG_NEXT64 || op > HWY_PCG_AT) return fail("%s", "hwy_debug_pcg64: unknown op");
+    if (n < 0) return fail("%s", "hwy_debug_pcg64: n < 0");
+    if (op == HWY_PCG_CHOICE && arg_i < 1) return fail("%s", "hwy_debug_pcg64: choice needs arg_i >= 1");
+    if (op == HWY_PCG_AT && (arg_i < 0 || arg_i >= hwy::kPcgJumpN))
+        return fail("%s", "hwy_debug_pcg64: pcg_at index outside the jump table");
+    if (op != HWY_PCG_AT && (count < 0 || count > (1 << 20))) return fail("%s", "hwy_debug_pcg64: count outside 0..2^20");
+    if (!words_in || !words_out || (op != HWY_PCG_AT && count > 0 && !draws))
+        return fail("%s", "hwy_debug_pcg64: null pointer");
+    if (n == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((op == HWY_PCG_AT || op == HWY_PCG_NORMAL) && ensure_pcg_jump(st)) return 1;
+    hwy::debug_pcg64_kernel<<<(n + 127) / 128, 128, 0, st>>>(op, arg_i, arg_lo, arg_hi, op == HWY_PCG_AT ? 0 : count,
+                                                              words_in, words_out, draws, n);
+    return check_launch("debug_pcg64_kernel");
 }
 
 int hwy_highway_autoreset(const HwyHighwayParams* p, const HwyHighwayState* s,

@@ -57,6 +57,8 @@ static __device__ __noinline__ double m_sin(double x) { return sin(x); }
 static __device__ __noinline__ double2 m_sincos_impl(double x) {
     const double ax = fabs(x);
     if (ax <= 0.7853981633974483) {
+        // fdlibm's |x| < 2^-27 shortcut: the polynomials round to (x, 1) there too, but would turn sin(-0.0) into +0.0
+        if (ax < 7.450580596923828e-09) return make_double2(x, 1.0);
         const double z = x * x;
         double r = fma(z, 1.58969099521155010221e-10, -2.50507602534068634195e-08);
         r = fma(z, r, 2.75573137070700676789e-06);
@@ -98,14 +100,16 @@ __device__ __forceinline__ double div_finite(double n, double d) { return n == 0
 // x ** delta of IDMVehicle.acceleration (behavior.py:183-186) for x >= 0.  DELTA = 4.0 unless randomize_behavior was
 // called: x^4 from two exact squarings (x*x = p + e and p*p = q + f with fma residuals), (p + e)^2 = q + f + 2pe + e^2
 // rounded once — within 0.51 ulp of the exact power, the quality of glibc's pow behind numpy's `**` (CUDA's pow is a
-// ~200-instruction routine with a 2 ulp bound).  Any other exponent, huge or non-finite x: the library pow.
+// ~200-instruction routine with a 2 ulp bound).  Below x^4 ~ 2^-968 (x < ~1e-73) the residuals are no longer exact
+// doubles: there the error is at most 0.5 ulp + 1.5 * 2^-1074 (<= 2 ulp in the lowest binade).  Any other exponent, huge or
+// non-finite x: the library pow.  tests/test_gpu_device_math.py measures these bounds on the device.
 //
 // randomize_behavior (highway-v0 / highway-fast-v0 traffic) draws DELTA from U(3.5, 4.5): then x^delta = x^4 * x^d with
 // |d| = |delta - 4| <= 0.5, the first factor as above and the second as exp(d * log(x)).  The usual weakness of
 // exp(y log x) — the error of log(x) is multiplied by y log x — is small here because |d log x| <= 0.35 for x in
 // [0.5, 2] (ratios of a speed to its target): ~1.5 ulp on top of the two functions' own 1 ulp, the same class as the
-// library pow's 2 ulp bound, and an absolute error below 1e-15 * x^delta for small x where (1 - x^delta) is what is
-// used.  It replaces ~175 issued instructions per call by ~80.  HWY_LIBRARY_POW restores the library call.
+// library pow's 2 ulp bound.  For small x the rounding of d * log(x) (|d log x| <= 69 down to x = 1e-60) dominates:
+// a relative error below 1e-14, irrelevant where (1 - x^delta) is what is used.  It replaces ~175 issued instructions per call by ~80.  HWY_LIBRARY_POW restores the library call.
 static __device__ __noinline__ double m_exp_dlog(double d, double x) { return exp(d * log(x)); }
 __device__ __forceinline__ double idm_pow(double x, double delta) {
 #ifndef HWY_LIBRARY_POW
@@ -129,7 +133,7 @@ __device__ __forceinline__ double idm_pow(double x, double delta) {
 
 
 // Python floored float modulo (b > 0 here).  fmod() is exact, so the cases around the principal range need no call:
-//   0 <= a < b      -> a
+//   0 <= a < b      -> |a|          (-0.0 % b is +0.0: fmod gives -0.0, then CPython's copysign(0, b))
 //   b <= a < 2b     -> a - b        (exact by Sterbenz: b <= a <= 2b)
 //   -b <= a < 0     -> fmod = a, then the sign fix-up `+= b` (one rounded add, as CPython's float_rem does)
 //   b == 1          -> a - floor(a) (exact) for a >= 0
@@ -145,7 +149,7 @@ static __device__ __noinline__ double py_mod_slow(double a, double b) {
 }
 __device__ __forceinline__ double py_mod_pos(double a, double b) {
     if (a >= 0.0) {
-        if (a < b) return a;
+        if (a < b) return fabs(a);
         if (a < b + b) return a - b;
         if (b == 1.0 && a < 4503599627370496.0) return a - floor(a);
     } else if (a >= -b) {

@@ -582,6 +582,27 @@ class BatchedRoundaboutEnv(ObservationHost):
         self._time.copy_(torch.from_numpy(np.asarray(sd["time"], dtype=np.float64).reshape(n)))
         if self._rngs is None:
             self._seed_streams(0)
+        if "rng" in sd:  # the env streams: [5][n] words, the layout of state_dict()["rng"]
+            w = np.ascontiguousarray(sd["rng"], dtype=np.uint64).reshape(5, n)
+            self._rng.copy_(torch.from_numpy(w.view(np.int64)).to(dev))
+            for e, g in enumerate(self._rngs):
+                g.bit_generator.state = {
+                    "bit_generator": "PCG64", "state": {"state": (int(w[0, e]) << 64) | int(w[1, e]),
+                                                        "inc": (int(w[2, e]) << 64) | int(w[3, e])},
+                    "has_uint32": int(w[4, e]) >> 32, "uinteger": int(w[4, e]) & 0xFFFFFFFF}
+
+    def rng_words(self) -> np.ndarray:
+        """The env streams as [5][n] words (state hi, lo, inc hi, lo, has_uint32 << 32 | uinteger): the device words
+        of reset_mode="device", the numpy generators' of the host-exact reset."""
+        if self.reset_mode == "device":
+            return self._rng.cpu().numpy().view(np.uint64).copy()
+        m = (1 << 64) - 1
+        w = np.zeros((5, self.num_envs), dtype=np.uint64)
+        for e, g in enumerate(self._rngs):
+            st = g.bit_generator.state
+            s, inc = st["state"]["state"], st["state"]["inc"]
+            w[:, e] = (s >> 64, s & m, inc >> 64, inc & m, (int(st["has_uint32"]) << 32) | int(st["uinteger"]))
+        return w
 
 
 class BatchedConnectedLaneRoundaboutEnv(BatchedRoundaboutEnv):

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define HWY_ABI_VERSION 13
+#define HWY_ABI_VERSION 14
 #define HWY_MAX_LANES 8
 #define HWY_MAX_TARGET_SPEEDS 8
 #define HWY_MAX_VEHICLES 128 /* per env, incl. the ego */
@@ -380,6 +380,35 @@ int hwy_intersection_reset(const HwyNetParams *p, const HwyNetGraph *graph, cons
 int hwy_debug_network_neighbours(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetState *s,
                                  const int32_t *query_lane, int32_t *front, int32_t *rear, void *stream);
 int hwy_debug_rotated_rectangles_intersect(const double *rects, int n, int32_t *out, void *stream);
+
+/* The scalar device functions of the step kernels (csrc/hwy_math.cuh, csrc/hwy_device.cuh) on n inputs, one thread
+ * each: in [n][k_in] and out [n][k_out] are DEVICE doubles; the operands of each op, in order, are
+ *   SINCOS x -> sin, cos (m_sincos)          IDM_POW x, delta -> x ** delta     EXP_DLOG d, x -> exp(d log x)
+ *   PY_MOD_POS a, b -> a % b (b > 0)         WRAP_TO_PI x                        NOT_ZERO x
+ *   DIV_FINITE n, d -> n / d                 DOT2 a0, a1, b0, b1 -> np.dot       NORM2 a0, a1 -> np.linalg.norm
+ *   BETA_CONTROLLED x -> sin, cos of the slip angle for the steering sine x (beta_of_controlled)
+ *   BETA_ANGLE delta -> sin, cos of arctan(tan(delta) / 2)
+ *   SPEED_TO_INDEX speed, n_target_speeds, target_speeds[HWY_MAX_TARGET_SPEEDS] -> index (as a double); NaN when
+ *                  n_target_speeds is not in 1..HWY_MAX_TARGET_SPEEDS. */
+enum {
+    HWY_MATH_SINCOS = 0, HWY_MATH_IDM_POW, HWY_MATH_EXP_DLOG, HWY_MATH_PY_MOD_POS, HWY_MATH_WRAP_TO_PI,
+    HWY_MATH_NOT_ZERO, HWY_MATH_DIV_FINITE, HWY_MATH_DOT2, HWY_MATH_NORM2, HWY_MATH_BETA_CONTROLLED,
+    HWY_MATH_BETA_ANGLE, HWY_MATH_SPEED_TO_INDEX
+};
+int hwy_debug_math(int op, const double *in, double *out, int n, void *stream);
+
+/* The numpy Generator(PCG64) restatement of the kernels, one generator per thread: words_in / words_out [5][n] in
+ * the HwyHighwayState.rng layout (DEVICE).  Each thread makes `count` draws of kind op into draws [n][count]
+ * (uint64; doubles as their IEEE bits): NEXT64, NEXT32, NEXT_DOUBLE, UNIFORM(arg_lo, arg_hi), CHOICE(arg_i) and
+ * NORMAL, which writes [n][count][2] = (value bits, 64-bit outputs the draw consumed; 0 when more than 16), then
+ * stores its generator in words_out.  AT positions the generator at output arg_i of its stream (the jump table of
+ * the fused autoreset, 0 <= arg_i < 4 * HWY_MAX_VEHICLES + 8) and draws nothing. */
+enum {
+    HWY_PCG_NEXT64 = 0, HWY_PCG_NEXT32, HWY_PCG_NEXT_DOUBLE, HWY_PCG_UNIFORM, HWY_PCG_NORMAL, HWY_PCG_CHOICE,
+    HWY_PCG_AT
+};
+int hwy_debug_pcg64(int op, int arg_i, double arg_lo, double arg_hi, int count, const uint64_t *words_in,
+                    uint64_t *words_out, uint64_t *draws, int n, void *stream);
 
 /* Road.act() + Road.step(dt) n_substeps times without an ego action, for the envs whose mask byte is
  * set (NULL: all): the 3 s warm-up of IntersectionEnv._make_vehicles (:271-278). */

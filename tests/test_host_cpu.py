@@ -19,7 +19,9 @@ def test_library_exports_every_declared_symbol():
     hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
     declared = set(re.findall(r"\b(hwy_[a-z_0-9]+)\s*\(", hdr))
     assert {"hwy_highway_step", "hwy_highway_reset", "hwy_highway_observe", "hwy_highway_autoreset",
-            "hwy_highway_slot_stride", "hwy_abi_version", "hwy_last_error", "hwy_launch_count"} <= declared
+            "hwy_highway_slot_stride", "hwy_abi_version", "hwy_last_error", "hwy_launch_count",
+            "hwy_debug_math", "hwy_debug_pcg64"} <= declared
+    assert declared <= set(N.EXPORTS) | {"hwy_debug_phase_cycles"}
     for sym in declared:
         assert getattr(lib, sym) is not None, sym
     assert lib.hwy_abi_version() == N.HWY_ABI_VERSION
@@ -61,6 +63,36 @@ def test_abi_validation_without_gpu():
     p.n_vehicles = 500
     assert lib.hwy_highway_observe(C.byref(p), C.byref(s), None, None) != 0
     assert b"n_vehicles" in lib.hwy_last_error()
+
+
+def test_test_entries_validate_their_arguments():
+    """hwy_debug_math / hwy_debug_pcg64 refuse bad ops, indices and pointers before touching the device."""
+    import ctypes as C
+
+    from highwayenv_b200 import _native as N
+
+    lib = N.load()
+    # host buffers for the pointer arguments a check does not concern: each call fails validation before any launch,
+    # and a regression in that order would hand a kernel a host pointer (a launch error), never a made-up address
+    buf = (C.c_double * 64)()
+    p = C.addressof(buf)
+    assert lib.hwy_debug_math(len(N.MATH_OPS), p, p, 4, None) != 0 and b"op" in lib.hwy_last_error()
+    assert lib.hwy_debug_math(-1, p, p, 4, None) != 0 and b"op" in lib.hwy_last_error()
+    assert lib.hwy_debug_math(0, p, None, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert lib.hwy_debug_math(0, None, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert lib.hwy_debug_math(0, p, p, -1, None) != 0 and b"n < 0" in lib.hwy_last_error()
+    assert lib.hwy_debug_math(0, None, None, 0, None) != 0
+    pcg = lib.hwy_debug_pcg64
+    assert pcg(len(N.PCG_OPS), 0, 0.0, 0.0, 1, p, p, p, 4, None) != 0 and b"op" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["pcg_at"], 4 * N.HWY_MAX_VEHICLES + 8, 0.0, 0.0, 0, p, p, None, 4, None) != 0
+    assert b"jump table" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["pcg_at"], -1, 0.0, 0.0, 0, p, p, None, 4, None) != 0
+    assert pcg(N.PCG_OPS["choice"], 0, 0.0, 0.0, 1, p, p, p, 4, None) != 0 and b"arg_i" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, -1, p, p, p, 4, None) != 0 and b"count" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, 1, None, p, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, 1, p, None, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["normal"], 0, 0.0, 0.0, 1, p, p, None, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, 1, p, p, p, -2, None) != 0 and b"n < 0" in lib.hwy_last_error()
 
 
 def test_default_configs_match_reference_values():
