@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HWYB200_LIB") or os.path.join(_HERE, "csrc", "libhwyb200.so")
 
@@ -147,6 +149,29 @@ class HwyMergeSpawn(C.Structure):
 
 KIND_OBSTACLE = 3
 META_NO_LANE_CHANGE = 1 << 23
+
+META_FLAG_BITS = {"crashed": META_CRASHED, "has_impact": META_HAS_IMPACT, "check_collisions": META_CHECK_COLLISIONS,
+                  "is_yielding": META_YIELDING, "no_lane_change": META_NO_LANE_CHANGE}
+
+
+def unpack_meta(meta, flags) -> dict:
+    """Per-vehicle meta words -> lane, target_lane, kind and the bool arrays of the named META_FLAG_BITS."""
+    meta = np.asarray(meta)
+    out = {"lane": (meta >> META_LANE_SHIFT) & 0xFF, "target_lane": (meta >> META_TARGET_SHIFT) & 0xFF,
+           "kind": (meta >> META_KIND_SHIFT) & 3}
+    for name in flags:
+        out[name] = (meta & META_FLAG_BITS[name]) != 0
+    return out
+
+
+def pack_meta(fields: dict, flags) -> np.ndarray:
+    """Inverse of unpack_meta for the named flags (every one of them must be in `fields`); sets META_PRESENT."""
+    meta = ((np.asarray(fields["lane"], dtype=np.int64) << META_LANE_SHIFT)
+            | (np.asarray(fields["target_lane"], dtype=np.int64) << META_TARGET_SHIFT)
+            | (np.asarray(fields["kind"], dtype=np.int64) << META_KIND_SHIFT) | META_PRESENT)
+    for name in flags:
+        meta = meta | np.where(np.asarray(fields[name], dtype=bool), META_FLAG_BITS[name], 0)
+    return meta.astype(np.int32)
 
 
 class HwyUTurnSpawn(C.Structure):

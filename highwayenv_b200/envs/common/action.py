@@ -123,6 +123,12 @@ class DiscreteAction(ContinuousAction):
         return Discrete(self.actions_per_axis ** 2)
 
 
+def speed_to_index(target_speeds, speed) -> int:
+    """MDPVehicle.speed_to_index (vehicle/controller.py): the index of the target speed closest to `speed`."""
+    ts = np.asarray(target_speeds, dtype=np.float64)
+    return int(np.clip(np.round((speed - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+
+
 ACTION_TYPES = {
     "DiscreteMetaAction": DiscreteMetaAction,
     "ContinuousAction": ContinuousAction,

@@ -21,10 +21,9 @@ class HostStepper:
     as a whole, so the host pays one launch for all of them."""
 
     def __init__(self, env) -> None:
-        seeded = env._seeded if hasattr(env, "_seeded") else getattr(env, "_rngs", None) is not None
-        if not seeded:
+        if not env._seeded:
             raise RuntimeError("call reset() before host_stepper()")
-        if getattr(env, "reset_mode", "device") != "device":
+        if env.reset_mode != "device":
             raise NotImplementedError("host_stepper needs the device reset path (reset_mode='device')")
         self.env = env
         dev = env.device

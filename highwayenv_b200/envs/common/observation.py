@@ -11,7 +11,7 @@ device observer:
   then runs the plugin's *standalone* kernel (``hwy_observe_grid`` / ``hwy_observe_ttc`` / ``hwy_observe_lidar``,
   include/hwyb200.h) on the device state — any plugin on any env, as in the reference.
 
-The env side of the contract is ``ObservationHost`` (the three hooks a family implements).
+The env side of the contract is ``BatchedVectorEnv._obs_view`` (envs/common/vector_env.py).
 """
 from __future__ import annotations
 
@@ -27,7 +27,7 @@ from ...spaces import Box
 class ObservationType:
     """Host-side descriptor of one observation plugin."""
 
-    standalone = False  # True: observed by its own kernel after the step (ObservationHost._observe_plugin)
+    standalone = False  # True: observed by its own kernel after the step (BatchedVectorEnv._observe_plugin)
 
     def space(self):
         raise NotImplementedError
@@ -234,12 +234,54 @@ def observation_factory(env, config: dict) -> ObservationType:
     raise ValueError("Unknown observation type")
 
 
-class ObservationHost:
-    """What an env family provides to the standalone plugins."""
+FUSED_TTC_MAX_T, FUSED_TTC_MAX_SPEEDS = 16, 3  # EnvStage's shared TimeToCollision grid (hwy_network.cu)
 
-    def _obs_view(self):
-        """-> (HwyObsView of the current state, device pointer of the HwyNetGraph lane table)"""
-        raise NotImplementedError
 
-    def _observe_plugin(self, out, mask_a=None, mask_b=None) -> None:
-        self.observation_type.observe(self, out, mask_a, mask_b)
+def select_network_observation(env, p: N.HwyNetParams, config: dict, target_speeds, ego_side_lanes: int,
+                               fuse_ttc: bool = True, fuse_grid: bool = True, feature_columns: bool = False):
+    """Select the plugin with the reference's factory rule for a network-kernel env and decide whether the step
+    kernel writes it itself (fused: Kinematics with 5 / 7 columns, or any columns with `feature_columns`; the default
+    OccupancyGrid with `fuse_grid`; TimeToCollision up to 16 time cells with `fuse_ttc`) or a standalone kernel runs
+    after the step.  Fills the observation fields of `p`; returns (plugin, fused)."""
+    plugin = observation_factory(env, config)
+    fused = False
+    if isinstance(plugin, TimeToCollisionObservation):
+        plugin.bind(p.policy_frequency, target_speeds)
+        n_t = plugin.horizon * p.policy_frequency
+        if fuse_ttc and n_t <= FUSED_TTC_MAX_T and p.n_target_speeds <= FUSED_TTC_MAX_SPEEDS:
+            p.obs_type, p.ttc_horizon, p.obs_vehicles_count, fused = N.OBS_TTC, plugin.horizon, 5, True
+    elif isinstance(plugin, OccupancyGridObservation):
+        if fuse_grid and plugin.is_default:
+            p.obs_type, p.obs_vehicles_count, fused = N.OBS_OCCUPANCY, 5, True
+    elif isinstance(plugin, KinematicObservation):
+        feats = plugin.features
+        if config.get("observe_intentions"):
+            raise NotImplementedError("Kinematics observe_intentions on the network kernels")
+        # normalize_obs (observation.py:214-226), computed at the first observation of an episode: the y-range spans
+        # all_side_lanes of the controlled vehicle's spawn road
+        w = 4.0 * ego_side_lanes
+        fr = plugin.features_range
+        if fr is None:
+            fr = {"x": [-5.0 * 40.0, 5.0 * 40.0], "y": [-w, w], "vx": [-2 * 40.0, 2 * 40.0], "vy": [-2 * 40.0, 2 * 40.0]}
+        if feats[:5] != ["presence", "x", "y", "vx", "vy"] or feats[5:] not in ([], ["cos_h", "sin_h"]):
+            if not feature_columns:
+                raise NotImplementedError(f"Kinematics features {feats} on the network kernels "
+                                          "(presence, x, y, vx, vy [, cos_h, sin_h])")
+            # any Vehicle.to_dict column list (vehicle/kinematics.py:237-261) with per-column ranges
+            p.obs_n_feat = len(feats)
+            for k, f in enumerate(feats):
+                p.obs_feat[k] = N.FEATURE_CODES[f]
+                if f in fr:
+                    p.obs_feat_ranged[k], p.obs_feat_lo[k], p.obs_feat_hi[k] = 1, float(fr[f][0]), float(fr[f][1])
+        p.obs_type, p.obs_features = N.OBS_KINEMATICS, len(feats)
+        p.obs_vehicles_count = plugin.vehicles_count
+        p.obs_see_behind, p.obs_absolute = int(plugin.see_behind), int(plugin.absolute)
+        p.obs_normalize, p.obs_clip = int(plugin.normalize), int(plugin.clip)
+        (p.obs_x_lo, p.obs_x_hi), (p.obs_y_lo, p.obs_y_hi) = (map(float, fr["x"]), map(float, fr["y"]))
+        (p.obs_vx_lo, p.obs_vx_hi), (p.obs_vy_lo, p.obs_vy_hi) = (map(float, fr["vx"]), map(float, fr["vy"]))
+        fused = True
+    if not fused:  # the kernels write one Kinematics row into a scratch buffer; the plugin observes after them
+        p.obs_type, p.obs_features, p.obs_vehicles_count = N.OBS_KINEMATICS, 5, 1
+        p.obs_x_lo = p.obs_y_lo = p.obs_vx_lo = p.obs_vy_lo = -1.0
+        p.obs_x_hi = p.obs_y_hi = p.obs_vx_hi = p.obs_vy_hi = 1.0
+    return plugin, fused

@@ -11,13 +11,11 @@ population changes); reset is ``hwy_exit_reset`` on the env's numpy stream (weig
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
-import torch
 
 from .. import _native as N
 from ..road.network import NetworkTable
+from .common.action import speed_to_index
 from .common.observation import OBSERVATION_TYPES, KinematicObservation
 from .roundabout_env import BatchedRoundaboutEnv
 
@@ -54,6 +52,7 @@ def make_exit_network(lanes_count: int = 6, road_length: float = 1000, exit_posi
 
 class BatchedExitEnv(BatchedRoundaboutEnv):
     ENV_ID = "exit-v0"
+    RESET_ENTRY = "hwy_exit_reset"
     SLOTS = N.HWY_NET_GROUP_LARGE
     N_VEHICLES = 21
     REWARD_NAMES = ("collision_reward", "goal_reward", "high_speed_reward", "right_lane_reward")  # _rewards :164-176
@@ -99,7 +98,7 @@ class BatchedExitEnv(BatchedRoundaboutEnv):
         s = N.HwyExitSpawn()
         s.lanes_count, s.n_vehicles = n_l, self.N_VEHICLES
         ts = self.action_type.target_speeds
-        s.ego_speed_index = int(np.clip(np.round((25.0 - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+        s.ego_speed_index = speed_to_index(ts, 25.0)
         s.ego_speed, s.ego_spacing = 25.0, float(cfg["ego_spacing"])
         s.vehicles_density = float(cfg["vehicles_density"])
         s.spawn_exp = float(np.exp(-5 / 40 * n_l))
@@ -113,16 +112,9 @@ class BatchedExitEnv(BatchedRoundaboutEnv):
         s.route_23 = int(net.encode_route([("2", "3", None)])[0][0])
         self._spawn_struct = s
 
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_exit_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
-
-    def step(self, actions):
-        out = super().step(actions)
-        out[4]["is_success"] = self._reward_terms[:, 1] > 0  # ExitEnv.step (:51-54): info["is_success"]
-        return out
+    def _step_result(self, info):
+        info["is_success"] = self._reward_terms[:, 1] > 0  # ExitEnv.step (:51-54): info["is_success"]
+        return super()._step_result(info)
 
 
 class BatchedConnectedLaneExitEnv(BatchedExitEnv):

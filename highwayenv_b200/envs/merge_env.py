@@ -10,14 +10,12 @@ x = 370 and is never truncated (:80-84).
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
-import torch
 
 from .. import _native as N
 from ..road.network import NetworkTable
 from ..spaces import Box
+from .common.action import speed_to_index
 from .roundabout_env import BatchedRoundaboutEnv
 
 
@@ -51,6 +49,7 @@ def make_merge_network() -> NetworkTable:
 
 class BatchedMergeEnv(BatchedRoundaboutEnv):
     ENV_ID = "merge-v0"
+    RESET_ENTRY = "hwy_merge_reset"
     N_VEHICLES = 6  # five vehicles + the Obstacle
     EGO_SIDE_LANES = 2  # the controlled vehicle spawns on ("a", "b", 1): normalize_obs' default y-range (observation.py:214-226)
     REWARD_NAMES = ("collision_reward", "right_lane_reward", "high_speed_reward", "lane_change_reward", "merging_speed_reward")  # _rewards :62-77
@@ -79,16 +78,10 @@ class BatchedMergeEnv(BatchedRoundaboutEnv):
         s.lane_ab[0], s.lane_ab[1] = net.index[("a", "b", 0)], net.index[("a", "b", 1)]
         s.lane_jk = net.index[("j", "k", 0)]
         ts = self.action_type.target_speeds
-        s.ego_speed_index = int(np.clip(np.round((30.0 - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+        s.ego_speed_index = speed_to_index(ts, 30.0)
         ox, oy = net.position(net.index[("b", "c", 2)], 80.0, 0.0)
         s.obstacle_x, s.obstacle_y = float(ox), float(oy)
         self._spawn_struct = s
-
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_merge_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
 
 
 class BatchedConnectedLaneMergeEnv(BatchedMergeEnv):

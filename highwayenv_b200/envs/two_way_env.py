@@ -8,13 +8,9 @@ is) (:35-55); terminated on a crash, never truncated (:57-62).  Same 8-slot kern
 """
 from __future__ import annotations
 
-import ctypes as C
-
-import numpy as np
-import torch
-
 from .. import _native as N
 from ..road.network import NetworkTable
+from .common.action import speed_to_index
 from .roundabout_env import BatchedRoundaboutEnv
 
 
@@ -30,6 +26,7 @@ def make_two_way_network(length: float = 800) -> NetworkTable:
 
 class BatchedTwoWayEnv(BatchedRoundaboutEnv):
     ENV_ID = "two-way-v0"
+    RESET_ENTRY = "hwy_two_way_reset"
     N_VEHICLES = 6
     EGO_SIDE_LANES = 2  # ("a", "b", 0 / 1)
     REWARD_NAMES = ("high_speed_reward", "left_lane_reward")  # _rewards :50-59
@@ -53,11 +50,5 @@ class BatchedTwoWayEnv(BatchedRoundaboutEnv):
         s = N.HwyTwoWaySpawn()
         s.lane_ab1, s.lane_ba0 = self.net.index[("a", "b", 1)], self.net.index[("b", "a", 0)]
         ts = self.action_type.target_speeds
-        s.ego_speed_index = int(np.clip(np.round((30.0 - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+        s.ego_speed_index = speed_to_index(ts, 30.0)
         self._spawn_struct = s
-
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_two_way_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))

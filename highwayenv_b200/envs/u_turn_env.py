@@ -8,13 +8,11 @@ on a crash, truncated at ``duration`` = 10 s.  Same 8-slot kernels as roundabout
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
-import torch
 
 from .. import _native as N
 from ..road.network import NetworkTable
+from .common.action import speed_to_index
 from .roundabout_env import BatchedRoundaboutEnv
 
 
@@ -37,6 +35,7 @@ def make_u_turn_network(length: float = 128) -> NetworkTable:
 
 class BatchedUTurnEnv(BatchedRoundaboutEnv):
     ENV_ID = "u-turn-v0"
+    RESET_ENTRY = "hwy_u_turn_reset"
     N_VEHICLES = 7
     EGO_SIDE_LANES = 2  # ("a", "b", 0 / 1)
     REWARD_NAMES = ("collision_reward", "left_lane_reward", "high_speed_reward", "on_road_reward")  # _rewards :61-72
@@ -60,27 +59,15 @@ class BatchedUTurnEnv(BatchedRoundaboutEnv):
 
     def _build_spawn_tables(self) -> None:
         net = self.net
-        n_l = len(net.lanes)
-        table = np.zeros((n_l, N.HWY_NET_MAX_ROUTE), dtype=np.int32)
-        lens = np.zeros(n_l, dtype=np.int32)
-        for l in range(n_l):  # plan_route_to("d") (vehicle/controller.py:71-87)
-            table[l], lens[l] = net.encode_route(net.plan_route(net.lane_index_of[l], "d"))
-        self._route_table = torch.from_numpy(table).to(self.device)
-        self._route_table_len = torch.from_numpy(lens).to(self.device)
+        self._route_tables(["d"])
         s = N.HwyUTurnSpawn()
         s.lane[0] = net.index[("a", "b", 0)]
         for k, (li, lon, speed) in enumerate(self.TRAFFIC, start=1):
             s.lane[k], s.longitudinal[k], s.speed[k] = net.index[li], lon, speed
         ts = self.action_type.target_speeds
-        s.ego_speed_index = int(np.clip(np.round((16.0 - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+        s.ego_speed_index = speed_to_index(ts, 16.0)
         s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
         self._spawn_struct = s
-
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_u_turn_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
 
 
 class BatchedConnectedLaneUTurnEnv(BatchedUTurnEnv):

@@ -200,6 +200,15 @@ class NetworkTable:
             enc[k] = self.node_id[f] | (self.node_id[t] << 8) | (((-1 if lid is None else int(lid)) + 1) << 16)
         return enc, len(route)
 
+    def route_table(self, destinations: Sequence[str]) -> Tuple[np.ndarray, np.ndarray]:
+        """The encoded plan_route(lane, destination) of every lane and destination: [lanes, D, MAX_ROUTE], [lanes, D]."""
+        table = np.zeros((len(self.lanes), len(destinations), N.HWY_NET_MAX_ROUTE), dtype=np.int32)
+        lens = np.zeros((len(self.lanes), len(destinations)), dtype=np.int32)
+        for l in range(len(self.lanes)):
+            for d, dest in enumerate(destinations):
+                table[l, d], lens[l, d] = self.encode_route(self.plan_route(self.lane_index_of[l], dest))
+        return table, lens
+
     # ------------------------------------------------------------------ vectorised lane geometry (host reset)
     def position(self, lane: int, s, lat):
         """lane.position(s, lat) for arrays s, lat (lane.py:192-197,268-273,338-342)."""

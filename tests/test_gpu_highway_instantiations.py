@@ -76,3 +76,8 @@ def test_host_stepper_discrete_action(env_id, over):
     hs.actions[0] = 9
     with pytest.raises(IndexError):
         hs.step()
+    for bad in (9, -1):  # the eager env.step path checks the index before its device gather
+        act = np.zeros(n, dtype=np.int64)
+        act[n // 2] = bad
+        with pytest.raises(IndexError):
+            a.step(act)

@@ -347,3 +347,64 @@ def test_gymnasium_registration_hook_registers_every_id(monkeypatch):
     assert len([k for k in registry if k.startswith("hwyb200/")]) == len(hb.REGISTRY)
     for name in [m for m in sys.modules if m == "gymnasium" or m.startswith("gymnasium.")]:
         sys.modules.pop(name, None)  # leave no stub behind for the tests that follow
+
+
+def test_pcg64_words_round_trip():
+    """The generator <-> device-word conversion against numpy's bit_generator.state, with and without a buffered
+    32-bit half."""
+    from highwayenv_b200.envs.common.vector_env import pcg64_words, set_pcg64_words
+
+    gens = [np.random.Generator(np.random.PCG64(np.random.SeedSequence(s))) for s in (0, 1, 2**63 + 5, 12345)]
+    gens[1].integers(0, 7, dtype=np.uint32)  # one 32-bit draw leaves the other half buffered
+    gens[2].normal(size=3)
+    gens[3].integers(0, 7, size=2, dtype=np.uint32)  # two: the buffer is used up again
+    states = [g.bit_generator.state for g in gens]
+    assert [st["has_uint32"] for st in states] == [0, 1, 0, 0]
+    words = pcg64_words(gens)
+    assert words.shape == (5, 4) and words.dtype == np.uint64
+    for i, st in enumerate(states):
+        w = [int(x) for x in words[:, i]]
+        assert (w[0] << 64) | w[1] == st["state"]["state"] and (w[2] << 64) | w[3] == st["state"]["inc"]
+        assert w[4] == (st["has_uint32"] << 32) | st["uinteger"]
+    fresh = [np.random.Generator(np.random.PCG64(9)) for _ in gens]
+    set_pcg64_words(fresh, words)
+    for g, h, st in zip(gens, fresh, states):
+        assert h.bit_generator.state == st
+        assert g.integers(0, 1 << 30, size=5, dtype=np.uint32).tolist() == h.integers(0, 1 << 30, size=5, dtype=np.uint32).tolist()
+    assert np.array_equal(pcg64_words(fresh), pcg64_words(gens))
+
+
+def test_meta_word_pack_round_trip():
+    """pack_meta / unpack_meta over every flag combination, lane, target lane and kind."""
+    import itertools
+
+    from highwayenv_b200 import _native as N
+
+    flags = tuple(N.META_FLAG_BITS)
+    combos = np.array(list(itertools.product([False, True], repeat=len(flags))))
+    m = len(combos)
+    fields = {"lane": np.arange(m) % 32, "target_lane": (np.arange(m) * 7) % 32, "kind": np.arange(m) % 4}
+    fields.update({f: combos[:, k] for k, f in enumerate(flags)})
+    meta = N.pack_meta(fields, flags)
+    assert meta.dtype == np.int32 and np.all(meta & N.META_PRESENT)
+    out = N.unpack_meta(meta, flags)
+    for k, v in fields.items():
+        assert np.array_equal(out[k], v), k
+    bits = [N.META_FLAG_BITS[f] for f in flags]
+    assert len(set(bits)) == len(bits) and not any(b & 0xFFFF or b & (3 << N.META_KIND_SHIFT) for b in bits)
+    assert not np.any(N.pack_meta(fields, ()) & sum(bits))  # only the named flags are packed
+
+
+def test_speed_to_index_matches_the_reference_formula():
+    """MDPVehicle.speed_to_index at the clip edges and at ties (np.round rounds half to even)."""
+    from highwayenv_b200.envs.common.action import speed_to_index
+
+    def reference(ts, v):
+        return int(np.clip(np.round((v - ts[0]) / (ts[-1] - ts[0]) * (ts.size - 1)), 0, ts.size - 1))
+
+    ts = np.linspace(20, 30, 3)
+    for v, want in ((-5.0, 0), (20.0, 0), (22.5, 0), (22.500001, 1), (25.0, 1), (27.5, 2), (30.0, 2), (99.0, 2)):
+        assert speed_to_index(ts, v) == want == reference(ts, v), v
+    for ts in (np.linspace(20, 30, 3), np.array([0.0, 10.0]), np.linspace(5, 6, 8), np.array([8.0, 16.0, 24.0, 32.0])):
+        for v in np.concatenate([ts, (ts[1:] + ts[:-1]) / 2, [ts[0] - 1, ts[-1] + 1, 8.0, 10.0, 16.0, 25.0, 30.0]]):
+            assert speed_to_index(ts, v) == reference(ts, v), (ts, v)
