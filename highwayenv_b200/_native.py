@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HWYB200_LIB") or os.path.join(_HERE, "csrc", "libhwyb200.so")
 
-HWY_ABI_VERSION = 14 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
+HWY_ABI_VERSION = 15 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
 HWY_MAX_LANES = 8
 HWY_MAX_TARGET_SPEEDS = 8
 HWY_MAX_VEHICLES = 128
@@ -229,6 +229,21 @@ class HwyTtcParams(C.Structure):
                 ("_pad", C.c_int32), ("target_speeds", C.c_double * HWY_MAX_TARGET_SPEEDS)]
 
 
+class HwyFiniteMdpParams(C.Structure):
+    _fields_ = [("policy_frequency", C.c_int32), ("n_target_speeds", C.c_int32), ("l_max", C.c_int32),
+                ("n_t", C.c_int32), ("horizon", C.c_double), ("target_speeds", C.c_double * HWY_MAX_TARGET_SPEEDS),
+                ("collision_reward", C.c_double), ("right_lane_reward", C.c_double), ("high_speed_reward", C.c_double),
+                ("lane_change_reward", C.c_double)]
+
+
+HWY_VI_MAX_STATES, HWY_VI_MAX_ACTIONS = 4096, 8
+
+
+class HwyValueIterationParams(C.Structure):
+    _fields_ = [("n_envs", C.c_int32), ("s_max", C.c_int32), ("n_actions", C.c_int32), ("iterations", C.c_int32),
+                ("gamma", C.c_double), ("state", C.c_void_p), ("action", C.c_void_p)]
+
+
 class HwyLidarParams(C.Structure):
     _fields_ = [("cells", C.c_int32), ("normalize", C.c_int32), ("maximum_range", C.c_double)]
 
@@ -240,7 +255,8 @@ EXPORTS = (
     "hwy_network_obs_size", "hwy_network_step", "hwy_network_observe", "hwy_roundabout_reset",
     "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset", "hwy_intersection_step_agents",
     "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
-    "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64",
+    "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
+    "hwy_value_iteration",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -332,6 +348,10 @@ def load():
     lib.hwy_observe_ttc.argtypes = [NG, OV, C.POINTER(HwyTtcParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_observe_lidar.restype = C.c_int
     lib.hwy_observe_lidar.argtypes = [OV, C.POINTER(HwyLidarParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_finite_mdp.restype = C.c_int
+    lib.hwy_finite_mdp.argtypes = [NG, OV, C.POINTER(HwyFiniteMdpParams)] + [C.c_void_p] * 8
+    lib.hwy_value_iteration.restype = C.c_int
+    lib.hwy_value_iteration.argtypes = [C.POINTER(HwyValueIterationParams)] + [C.c_void_p] * 7
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

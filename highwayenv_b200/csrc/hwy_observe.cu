@@ -232,36 +232,21 @@ __device__ bool is_connected_road(const GraphShared& g, int f1, int t1, int f2, 
 }
 
 constexpr int kTtcMaxLanes = 8, kTtcMaxT = 64;
+typedef int TtcCost2[HWY_MAX_TARGET_SPEEDS][kTtcMaxLanes][kTtcMaxT];  // 2 * cost (0, 1 = 0.5, 2 = 1.0)
 
-// envs/common/finite_mdp.py:104-163 compute_ttc_grid + observation.py:128-152 (pad with ones, crop 3 x 3)
-__global__ void __launch_bounds__(kThreads)
-ttc_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObsView view,
-           const __grid_constant__ HwyTtcParams P, const uint8_t* __restrict__ mask_a,
-           const uint8_t* __restrict__ mask_b, float* __restrict__ obs) {
-    __shared__ GraphShared g;
-    __shared__ int cost2[HWY_MAX_TARGET_SPEEDS][kTtcMaxLanes][kTtcMaxT];  // 2 * cost (0, 1 = 0.5, 2 = 1.0)
-    __shared__ int s_ego;
-    const int A = view.n_agents > 1 ? view.n_agents : 1;
-    const int e = blockIdx.x / A, agent = blockIdx.x % A;
-    if (!env_selected(mask_a, mask_b, e)) return;
-    stage_graph(g, graph);
-    const int tid = threadIdx.x;
-    const int count = view.count ? view.count[e] : view.n_vehicles;
-    if (tid == 0) s_ego = find_ego(view, e, count, agent);
-    for (int k = tid; k < HWY_MAX_TARGET_SPEEDS * kTtcMaxLanes * kTtcMaxT; k += kThreads) (&cost2[0][0][0])[k] = 0;
-    __syncthreads();
-    const int ego_slot = s_ego;
-    const Veh ego = load_veh(view, e, ego_slot);
-    const HwyNetLane& EL = g.lanes[ego.lane];
-    const int n_speeds = P.n_target_speeds, n_lanes = EL.road_count;
-    const double tq = 1.0 / P.policy_frequency;
-    const int n_t = (int)(P.horizon / tq);
+// envs/common/finite_mdp.py:104-163 compute_ttc_grid of env e, observed by the vehicle in `ego_slot`, into the
+// zeroed shared `cost2` with n_t cells of tq seconds; all lanes of the ego's road (EL).  Called by every thread of
+// the block; the caller synchronises before reading cost2.
+__device__ void ttc_grid_accumulate(const GraphShared& g, const HwyObsView& view, int e, int count, int ego_slot,
+                                    const Veh& ego, const HwyNetLane& EL, int n_speeds, const double* target_speeds,
+                                    double tq, int n_t, TtcCost2& cost2) {
+    const int n_lanes = EL.road_count;
     double es, ec;
     m_sincos(ego.heading, &es, &ec);
     const double ego_s = lane_s_of(EL, ego.x, ego.y);
     const int* route = view.route ? view.route + ((size_t)e * view.vp + ego_slot) * R : nullptr;
     const int rlen = view.route_len ? view.route_len[(size_t)e * view.vp + ego_slot] : 0;
-    for (int s = tid; s < count; s += kThreads) {
+    for (int s = threadIdx.x; s < count; s += blockDim.x) {
         if (s == ego_slot) continue;
         const Veh o = load_veh(view, e, s);
         if (o.kind == HWY_KIND_OBSTACLE) continue;  // road.vehicles only
@@ -273,7 +258,7 @@ ttc_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObs
         m_sincos(o.heading, &os, &oc);
         const double other_projected_speed = o.speed * dot2(oc, os, ec, es);
         for (int si = 0; si < n_speeds; ++si) {
-            const double ego_speed = P.target_speeds[si];
+            const double ego_speed = target_speeds[si];
             if (ego_speed == o.speed) continue;
             for (int k = 0; k < 3; ++k) {
                 const double m = k == 0 ? 0.0 : (k == 1 ? -margin : margin);
@@ -293,6 +278,32 @@ ttc_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObs
             }
         }
     }
+}
+
+// compute_ttc_grid + observation.py:128-152 (pad with ones, crop 3 x 3)
+__global__ void __launch_bounds__(kThreads)
+ttc_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObsView view,
+           const __grid_constant__ HwyTtcParams P, const uint8_t* __restrict__ mask_a,
+           const uint8_t* __restrict__ mask_b, float* __restrict__ obs) {
+    __shared__ GraphShared g;
+    __shared__ TtcCost2 cost2;
+    __shared__ int s_ego;
+    const int A = view.n_agents > 1 ? view.n_agents : 1;
+    const int e = blockIdx.x / A, agent = blockIdx.x % A;
+    if (!env_selected(mask_a, mask_b, e)) return;
+    stage_graph(g, graph);
+    const int tid = threadIdx.x;
+    const int count = view.count ? view.count[e] : view.n_vehicles;
+    if (tid == 0) s_ego = find_ego(view, e, count, agent);
+    for (int k = tid; k < HWY_MAX_TARGET_SPEEDS * kTtcMaxLanes * kTtcMaxT; k += kThreads) (&cost2[0][0][0])[k] = 0;
+    __syncthreads();
+    const int ego_slot = s_ego;
+    const Veh ego = load_veh(view, e, ego_slot);
+    const HwyNetLane& EL = g.lanes[ego.lane];
+    const int n_speeds = P.n_target_speeds, n_lanes = EL.road_count;
+    const double tq = 1.0 / P.policy_frequency;
+    const int n_t = (int)(P.horizon / tq);
+    ttc_grid_accumulate(g, view, e, count, ego_slot, ego, EL, n_speeds, P.target_speeds, tq, n_t, cost2);
     __syncthreads();
     const int speed_index = view.speed_index ? view.speed_index[(size_t)e * A + agent] : 0;
     float* out = obs + ((size_t)e * A + agent) * (size_t)(9 * n_t);
@@ -304,6 +315,79 @@ ttc_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObs
         const int lcol = n_lanes + EL.lane_id - 1 + b;
         const float val = (lcol < n_lanes || lcol >= 2 * n_lanes) ? 1.0f : 0.5f * (float)cost2[src][lcol - n_lanes][t];
         out[k] = val;
+    }
+}
+
+// ------------------------------------------------------------------ finite MDP (finite_mdp.py:17-101, 166-203)
+// finite_mdp(env, time_quantization=1/policy_frequency, horizon) of every env: the uncropped TTC grid of the first
+// controlled vehicle over the n_lanes = road_count lanes of its road, and the deterministic MDP on the raveled
+// (speed, lane, time) cells of that grid.  Rows s >= n_states of the [s_max] padding are absorbing: self-loops,
+// reward 0, terminal.
+__global__ void __launch_bounds__(kThreads)
+finite_mdp_kernel(const HwyNetGraph* __restrict__ graph, const __grid_constant__ HwyObsView view,
+                  const __grid_constant__ HwyFiniteMdpParams P, double* __restrict__ grid_out,
+                  int32_t* __restrict__ n_lanes_out, int32_t* __restrict__ n_states_out, int64_t* __restrict__ state_out,
+                  int32_t* __restrict__ transition, double* __restrict__ reward, uint8_t* __restrict__ terminal) {
+    __shared__ GraphShared g;
+    __shared__ TtcCost2 cost2;
+    __shared__ int s_ego;
+    const int e = blockIdx.x;
+    stage_graph(g, graph);
+    const int tid = threadIdx.x;
+    const int count = view.count ? view.count[e] : view.n_vehicles;
+    if (tid == 0) s_ego = find_ego(view, e, count, 0);
+    for (int k = tid; k < HWY_MAX_TARGET_SPEEDS * kTtcMaxLanes * kTtcMaxT; k += kThreads) (&cost2[0][0][0])[k] = 0;
+    __syncthreads();
+    const int ego_slot = s_ego;
+    const Veh ego = load_veh(view, e, ego_slot);
+    const HwyNetLane& EL = g.lanes[ego.lane];
+    const int V = P.n_target_speeds, T = P.n_t, LM = P.l_max;
+    const int L = EL.road_count < LM ? EL.road_count : LM;  // l_max covers every road of the graph (host-checked)
+    ttc_grid_accumulate(g, view, e, count, ego_slot, ego, EL, V, P.target_speeds, 1.0 / P.policy_frequency, T, cost2);
+    __syncthreads();
+    const int S = V * L * T, s_max = V * LM * T;
+    if (tid == 0) {
+        const int speed_index = view.speed_index ? view.speed_index[e] : 0;
+        n_lanes_out[e] = L;
+        n_states_out[e] = S;
+        state_out[e] = ((long long)speed_index * L + EL.lane_id) * T;  // ravel_multi_index((h, lane_index[2], 0))
+    }
+    double* ge = grid_out + (size_t)e * s_max;
+    for (int k = tid; k < s_max; k += kThreads) {
+        const int h = k / (LM * T), l = (k / T) % LM, t = k % T;
+        ge[k] = l < L ? 0.5 * cost2[h][l][t] : 0.0;
+    }
+    // state_reward = (collision * grid + right_lane * lanes) + high_speed * speeds;  reward = state_reward[s] +
+    // [lane_change, 0, lane_change, 0, 0][a]  (the reference's operation order; -fmad=false keeps each rounding)
+    const double lane_den = (double)(L - 1 > 1 ? L - 1 : 1), speed_den = (double)(V - 1 > 1 ? V - 1 : 1);
+    int32_t* tr = transition + (size_t)e * s_max * 5;
+    double* rw = reward + (size_t)e * s_max * 5;
+    uint8_t* te = terminal + (size_t)e * s_max;
+    for (int s = tid; s < s_max; s += kThreads) {
+        if (s >= S) {
+            for (int a = 0; a < 5; ++a) {
+                tr[s * 5 + a] = s;
+                rw[s * 5 + a] = 0.0;
+            }
+            te[s] = 1;
+            continue;
+        }
+        const int h = s / (L * T), i = (s / T) % L, j = s % T;
+        const double cell = 0.5 * cost2[h][i][j];
+        const double sr = (P.collision_reward * cell + P.right_lane_reward * ((double)i / lane_den)) +
+                          P.high_speed_reward * ((double)h / speed_den);
+        te[s] = cell == 1.0 || j == T - 1;
+        // transition_model / clip_position: every action advances time; LANE_LEFT / LANE_RIGHT move one lane,
+        // FASTER / SLOWER one speed only from the first time cell
+        const int jn = j + 1 < T ? j + 1 : T - 1;
+        const int il = i > 0 ? i - 1 : 0, ir = i + 1 < L ? i + 1 : L - 1;
+        const int hf = j == 0 && h + 1 < V ? h + 1 : h, hs = j == 0 && h > 0 ? h - 1 : h;
+        const int next[5] = {(h * L + il) * T + jn, (h * L + i) * T + jn, (h * L + ir) * T + jn, (hf * L + i) * T + jn,
+                             (hs * L + i) * T + jn};
+        for (int a = 0; a < 5; ++a) {
+            tr[s * 5 + a] = next[a];
+            rw[s * 5 + a] = sr + ((a == 0 || a == 2) ? P.lane_change_reward : 0.0);
+        }
     }
 }
 
@@ -473,6 +557,23 @@ int hwy_observe_ttc(const HwyNetGraph* graph, const HwyObsView* view, const HwyT
     hwyobs::ttc_kernel<<<view->n_envs * agents_of(view), hwyobs::kThreads, 0, (cudaStream_t)stream>>>(
         graph, *view, *p, mask_a, mask_b, obs);
     return check_launch("observe ttc_kernel");
+}
+
+int hwy_finite_mdp(const HwyNetGraph* graph, const HwyObsView* view, const HwyFiniteMdpParams* p, double* grid,
+                   int32_t* n_lanes, int32_t* n_states, int64_t* state, int32_t* transition, double* reward,
+                   uint8_t* terminal, void* stream) {
+    if (validate_view(view)) return 1;
+    if (!graph || !p || !grid || !n_lanes || !n_states || !state || !transition || !reward || !terminal)
+        return fail("%s", "null pointer");
+    if (view->n_agents > 1) return fail("%s", "finite MDP of a multi-agent env");
+    if (p->n_target_speeds < 1 || p->n_target_speeds > HWY_MAX_TARGET_SPEEDS) return fail("%s", "n_target_speeds out of range");
+    if (p->l_max < 1 || p->l_max > hwyobs::kTtcMaxLanes) return fail("%s", "l_max out of range (1..8)");
+    if (p->policy_frequency < 1 || !(p->horizon > 0)) return fail("%s", "bad horizon / policy_frequency");
+    if (p->n_t != (int)(p->horizon / (1.0 / p->policy_frequency))) return fail("%s", "n_t != int(horizon / (1 / policy_frequency))");
+    if (p->n_t < 1 || p->n_t > hwyobs::kTtcMaxT) return fail("%s", "n_t out of range (1..64)");
+    hwyobs::finite_mdp_kernel<<<view->n_envs, hwyobs::kThreads, 0, (cudaStream_t)stream>>>(
+        graph, *view, *p, grid, n_lanes, n_states, state, transition, reward, terminal);
+    return check_launch("finite_mdp_kernel");
 }
 
 int hwy_observe_lidar(const HwyObsView* view, const HwyLidarParams* p, const uint8_t* mask_a, const uint8_t* mask_b,

@@ -241,6 +241,14 @@ class BatchedVectorEnv:
             self._observe_plugin(self._obs)
         return self._out_obs()
 
+    def to_finite_mdp(self):
+        """AbstractEnv.to_finite_mdp() (envs/common/abstract.py:452-453) of every env, built on the device: the
+        time-to-collision MDP of highwayenv_b200.planning.FiniteMdp (`.env(i)` gives env i as the reference's
+        DeterministicMDP)."""
+        from ...planning import to_finite_mdp
+
+        return to_finite_mdp(self)
+
     def _observe_plugin(self, out, mask_a=None, mask_b=None) -> None:
         self.observation_type.observe(self, out, mask_a, mask_b)
 

@@ -74,5 +74,11 @@ class SingleEnv(_Base):
         mask = self.batched.get_available_actions()[0].cpu().numpy()
         return [int(i) for i in np.nonzero(mask)[0]]
 
+    def to_finite_mdp(self):
+        """AbstractEnv.to_finite_mdp() (envs/common/abstract.py:452-453): the time-to-collision MDP of the current
+        state with finite_mdp's DeterministicMDP attributes (transition, reward, terminal, state, original_shape,
+        mode), as rl-agents' ValueIterationAgent reads it from `env.unwrapped`."""
+        return self.batched.to_finite_mdp().env(0)
+
     def close(self) -> None:
         self.batched.close()

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define HWY_ABI_VERSION 14
+#define HWY_ABI_VERSION 15
 #define HWY_MAX_LANES 8
 #define HWY_MAX_TARGET_SPEEDS 8
 #define HWY_MAX_VEHICLES 128 /* per env, incl. the ego */
@@ -544,6 +544,45 @@ typedef struct HwyTtcParams {
 } HwyTtcParams;
 int hwy_observe_ttc(const HwyNetGraph *graph, const HwyObsView *view, const HwyTtcParams *p, const uint8_t *mask_a,
                     const uint8_t *mask_b, float *obs, void *stream);
+
+/* AbstractEnv.to_finite_mdp() = finite_mdp(env, time_quantization=1 / policy_frequency, horizon)
+ * (envs/common/abstract.py:452-453, envs/common/finite_mdp.py:17-203) of every env (one controlled vehicle, an
+ * MDPVehicle with 5 DiscreteMetaAction actions).  With V = n_target_speeds, L_e = lanes of the ego's road,
+ * T = n_t = int(horizon / (1 / policy_frequency)) and S_max = V * l_max * T (l_max >= every road's lane count):
+ *   grid [n_envs][V][l_max][T] f64 compute_ttc_grid (lanes >= L_e: 0);  n_lanes, n_states [n_envs] i32 (L_e, V*L_e*T);
+ *   state [n_envs] i64 ravel_multi_index((speed_index, lane_index[2], 0), (V, L_e, T));
+ *   transition [n_envs][S_max][5] i32, reward [n_envs][S_max][5] f64, terminal [n_envs][S_max] u8, raveled in each
+ *   env's own (V, L_e, T) shape; rows s >= n_states are self-loops with reward 0, terminal. */
+typedef struct HwyFiniteMdpParams {
+    int32_t policy_frequency, n_target_speeds;
+    int32_t l_max, n_t;
+    double horizon;
+    double target_speeds[HWY_MAX_TARGET_SPEEDS];
+    double collision_reward, right_lane_reward, high_speed_reward, lane_change_reward;
+} HwyFiniteMdpParams;
+int hwy_finite_mdp(const HwyNetGraph *graph, const HwyObsView *view, const HwyFiniteMdpParams *p, double *grid,
+                   int32_t *n_lanes, int32_t *n_states, int64_t *state, int32_t *transition, double *reward,
+                   uint8_t *terminal, void *stream);
+
+/* Value iteration of n_envs deterministic MDPs (the semantics of rl-agents' ValueIterationAgent), one block per
+ * env: Q_0 = 0; Q_new = reward + gamma * (terminal[s] ? 0 : max_a Q_k[transition[s, a]]); stop at the first k with
+ * np.allclose(Q_k, Q_new) over the env's n_states rows (keeping Q_k) or after `iterations` updates.
+ * transition [n_envs][s_max][n_actions] i32, reward f64, terminal [n_envs][s_max] u8, n_states [n_envs] i32;
+ * q [n_envs][s_max][n_actions] f64 (rows >= n_states: 0), iterations_done [n_envs] i32 = updates in q, or -1 when
+ * n_states is outside 0..s_max or a successor is outside 0..n_states-1 (q then stays 0).  With state [n_envs] i64
+ * and action [n_envs] i64 (both or neither), action[e] = the first argmax of q[e][state[e]] (-1 when the env
+ * failed or state is out of range).  s_max <= HWY_VI_MAX_STATES, n_actions <= HWY_VI_MAX_ACTIONS. */
+#define HWY_VI_MAX_STATES 4096
+#define HWY_VI_MAX_ACTIONS 8
+typedef struct HwyValueIterationParams {
+    int32_t n_envs, s_max, n_actions, iterations;
+    double gamma;
+    const int64_t *state; /* DEVICE or NULL */
+    int64_t *action;      /* DEVICE or NULL */
+} HwyValueIterationParams;
+int hwy_value_iteration(const HwyValueIterationParams *p, const int32_t *transition, const double *reward,
+                        const uint8_t *terminal, const int32_t *n_states, double *q, int32_t *iterations_done,
+                        void *stream);
 
 /* LidarObservation (observation.py:678-769): obs [n_envs][agents][cells][2] float32 (distance, relative radial speed) */
 typedef struct HwyLidarParams {
