@@ -70,6 +70,14 @@ class HwyHighwayState(C.Structure):
     ]
 
 
+HWY_LINEAR_PARAMS = 5
+
+
+class HwyLinearTraffic(C.Structure):
+    """LinearVehicle traffic of the highway family (include/hwyb200.h)."""
+    _fields_ = [("params", C.c_void_p), ("acc_lo", C.c_double * 3), ("acc_span", C.c_double * 3),
+                ("steer_lo", C.c_double * 2), ("steer_span", C.c_double * 2)]
+
 
 # ---- general road networks (roundabout-v0)
 HWY_NET_MAX_LANES, HWY_NET_MAX_NODES, HWY_NET_MAX_SUCC, HWY_NET_MAX_ROUTE, HWY_NET_GROUP = 32, 64, 6, 16, 8
@@ -256,7 +264,8 @@ EXPORTS = (
     "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset", "hwy_intersection_step_agents",
     "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
-    "hwy_value_iteration",
+    "hwy_value_iteration", "hwy_highway_linear_reset", "hwy_highway_linear_step", "hwy_highway_linear_autoreset",
+    "hwy_highway_linear_substeps",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -299,6 +308,15 @@ def load():
     lib.hwy_highway_substeps.argtypes = [P, S, C.c_int, C.c_void_p, C.c_void_p]
     lib.hwy_highway_autoreset.restype = C.c_int
     lib.hwy_highway_autoreset.argtypes = [P, S, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    T = C.POINTER(HwyLinearTraffic)
+    lib.hwy_highway_linear_reset.restype = C.c_int
+    lib.hwy_highway_linear_reset.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_highway_linear_step.restype = C.c_int
+    lib.hwy_highway_linear_step.argtypes = [P, S, T] + lib.hwy_highway_step.argtypes[2:]
+    lib.hwy_highway_linear_substeps.restype = C.c_int
+    lib.hwy_highway_linear_substeps.argtypes = [P, S, T, C.c_int, C.c_void_p, C.c_void_p]
+    lib.hwy_highway_linear_autoreset.restype = C.c_int
+    lib.hwy_highway_linear_autoreset.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     NP, NG, NS = C.POINTER(HwyNetParams), C.c_void_p, C.POINTER(HwyNetState)
     lib.hwy_network_obs_size.restype = C.c_int
     lib.hwy_network_obs_size.argtypes = [NP]

@@ -11,7 +11,7 @@ import sys
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(_HERE, "csrc", f) for f in ("hwy_highway.cu", "hwy_network.cu", "hwy_observe.cu", "hwy_plan.cu")]
-DEPS = SRC + [os.path.join(_HERE, "csrc", h) for h in ("hwy_math.cuh", "hwy_device.cuh", "hwy_lanes.cuh", "hwy_abi.h")] + [
+DEPS = SRC + [os.path.join(_HERE, "csrc", h) for h in ("hwy_math.cuh", "hwy_device.cuh", "hwy_lanes.cuh", "hwy_abi.h", "hwy_highway_step.cuh", "hwy_highway_reset.cuh")] + [
     os.path.join(os.path.dirname(_HERE), "include", "hwyb200.h")]
 OUT = os.path.join(_HERE, "csrc", "libhwyb200.so")
 

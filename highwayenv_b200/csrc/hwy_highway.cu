@@ -244,6 +244,51 @@ __device__ __forceinline__ double idm_acceleration_of(const HwyHighwayParams& P,
     return acc;
 }
 
+// ------------------------------------------------------------------ LinearVehicle (vehicle/behavior.py:350-583)
+// Per-env shared staging of the traffic's linear parameters, placed after the block's EnvShared array by the linear
+// kernel only (so EnvShared and the IDM kernel keep their layout): MOBIL items read the item owner's parameters.
+template <int TPE>
+struct LinearShared {
+    double acc[3][TPE];    // ACCELERATION_PARAMETERS
+    double steer[2][TPE];  // STEERING_PARAMETERS
+};
+
+// python min(x, 0): x unless 0 < x
+__device__ __forceinline__ double py_min0(double x) { return 0.0 < x ? 0.0 : x; }
+
+// :417-465 acceleration(ego_vehicle=ego, front_vehicle=front) with the CALLER's parameters (a0, a1, a2):
+// np.dot(ACCELERATION_PARAMETERS, [vt, dv, dp]), which numpy's BLAS evaluates as fma(a2, dp, fma(a1, dv, a0 * vt)).
+// F.ts holds getattr(ego, "target_speed", ego.speed) (publish<..., true>).
+template <int TPE>
+__device__ __forceinline__ double linear_acceleration(const HwyHighwayParams& P, const IdmK& K, const Frame<TPE>& F,
+                                                      bool aligned, double a0, double a1, double a2, int ego,
+                                                      int front) {
+    if (ego < 0) return 0.0;
+    const double v = F.v[ego];
+    const double vt = F.ts[ego] - v;
+    double dv = 0.0, dp = 0.0;
+    if (front >= 0) {
+        const double d_safe = K.distance_wanted + fmax(v, 0.0) * K.time_wanted;
+        const double d = lane_distance(P, F, aligned, ego, front);
+        dv = py_min0(F.v[front] - v);
+        dp = py_min0(d - d_safe);
+    }
+    return __fma_rn(a2, dp, __fma_rn(a1, dv, a0 * vt));
+}
+
+// :467-502 steering_control(target_lane) on a StraightLane (heading_at is the lane heading), then IDMVehicle.act's
+// clip to +-MAX_STEERING_ANGLE (:107-110); np.dot on the 2 features is fma(s1, f1, s0 * f0).
+static __device__ __noinline__ double linear_steering(const HwyStraightLane L, double x, double y, double heading,
+                                                      double speed, double s0, double s1) {
+    double lc_s, lc_lat;
+    lane_local(L, x, y, lc_s, lc_lat);
+    const double nz = not_zero(speed);
+    const double f0 = wrap_to_pi(L.heading - heading) * kVehLength / nz;
+    // (not_zero(v) ** 2 is the host libm's pow there, which can differ from the exact-rounded nz * nz by 1 ulp)
+    const double f1 = -lc_lat * kVehLength / (nz * nz);
+    return clipd(__fma_rn(s1, f1, s0 * f0), -kMaxSteer, kMaxSteer);
+}
+
 // ------------------------------------------------------------------ observation
 // envs/common/observation.py:234-276 KinematicObservation.observe (presence,x,y,vx,vy; order
 // "sorted") with road/road.py:421-450 close_objects_to and kinematics.py:237-261 to_dict.
@@ -409,7 +454,7 @@ __device__ __forceinline__ void store_vehicle(const HwyHighwayState& S, size_t s
 
 // Stage one vehicle into frame F (plain stores) and clear the words of F that build_frame fills
 // with atomics.  Callers put a barrier between publish() and build_frame().
-template <int TPE>
+template <int TPE, bool LINEAR = false>
 __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F, int i, bool active,
                                         const VehicleRegs& r) {
     constexpr int NW = TPE / 32;
@@ -421,8 +466,9 @@ __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F
         F.c[i] = cs;
         F.s[i] = sn;
         F.v[i] = r.speed;
-        // getattr(ego_vehicle, "target_speed", 0): a plain Vehicle has none (behavior.py:172)
-        F.ts[i] = meta_kind(r.meta) == HWY_KIND_VEHICLE ? 0.0 : r.target_speed;
+        // getattr(ego_vehicle, "target_speed", 0): a plain Vehicle has none (behavior.py:172); the linear model's
+        // default is the vehicle's own speed (behavior.py:449-452)
+        F.ts[i] = meta_kind(r.meta) == HWY_KIND_VEHICLE ? (LINEAR ? r.speed : 0.0) : r.target_speed;
         F.ls[i] = lane_s(P.lanes[0], r.x, r.y);
         F.lsf[i] = (float)F.ls[i];
         F.lane[i] = (unsigned char)meta_lane(r.meta);
@@ -773,6 +819,22 @@ __device__ __forceinline__ Pcg64 pcg_at(const Pcg64& g0, int n) {
     g.u32 = 0;
     return g;
 }
+// the same for any n >= 0: jumps of at most kPcgJumpN - 1 outputs (the linear traffic's spawn reaches ~1 100)
+__device__ __forceinline__ Pcg64 pcg_at_far(const Pcg64& g0, int n) {
+    Pcg64 g = g0;
+    while (n >= kPcgJumpN) {
+        g = pcg_at(g, kPcgJumpN - 1);
+        n -= kPcgJumpN - 1;
+    }
+    return pcg_at(g, n);
+}
+
+// LinearVehicle.randomize_behavior (behavior.py:406-415) before the inherited DELTA draw: uniform(size=3), then
+// uniform(size=2) — each element 0.0 + 1.0 * next_double — mapped by RANGE[0] + u * (RANGE[1] - RANGE[0]).
+__device__ __forceinline__ void draw_linear_params(Pcg64& g, const HwyLinearTraffic& T, double (&p)[HWY_LINEAR_PARAMS]) {
+    for (int k = 0; k < 3; ++k) p[k] = T.acc_lo[k] + g.next_double() * T.acc_span[k];
+    for (int k = 0; k < 2; ++k) p[3 + k] = T.steer_lo[k] + g.next_double() * T.steer_span[k];
+}
 
 // HighwayEnv._create_vehicles (envs/highway_env.py:72-98,177-182) for one env inside the step
 // kernel, one vehicle per thread.  Vehicle.create_random (vehicle/kinematics.py:50-104) draws,
@@ -784,15 +846,20 @@ __device__ __forceinline__ Pcg64 pcg_at(const Pcg64& g0, int n) {
 // rounds like the reference).  Rejections, or lanes that are not the x-aligned highway, fall
 // back to the serial draw order on one thread.  All threads of the BLOCK must call this
 // (barriers); only envs with do_reset do work.  On return r/speed_index hold the new state.
-template <int TPE>
+// LINEAR: LinearVehicle traffic draws its 5 parameters between the position and DELTA (8 outputs per
+// vehicle instead of 3) and stores them in T->params.
+template <int TPE, bool LINEAR = false>
 __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const HwyHighwayState& S,
                                             EnvShared<TPE>& sm, int e, int i, bool active,
                                             bool do_reset, bool simple_geometry, VehicleRegs& r,
-                                            int& speed_index) {
+                                            int& speed_index, const HwyLinearTraffic* T = nullptr) {
     const int V = P.n_vehicles, L = P.lanes_count;
     const size_t n = (size_t)S.n_envs;
+    constexpr int kPer = LINEAR ? 3 + HWY_LINEAR_PARAMS : 3;  // 64-bit outputs per traffic vehicle
+    auto jump = [](const Pcg64& g, int k) { return LINEAR ? pcg_at_far(g, k) : pcg_at(g, k); };
     Pcg64 g0;
     double speed = 0.0, delta = 4.0, incr = 0.0;
+    double lin[HWY_LINEAR_PARAMS] = {0.0, 0.0, 0.0, 0.0, 0.0};
     int lane_id = 0;
     if (do_reset) {
         g0.s_hi = S.rng[0 * n + e];
@@ -807,13 +874,13 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
     const int n32 = L > 1 ? 1 : 0;                            // choice(1) draws nothing
     const int ego32 = (n32 && P.initial_lane_id < 0) ? 1 : 0;
     auto q_before = [&](int k) { return k == 0 ? 0 : ego32 + (k - 1) * n32; };       // 32-bit requests before k
-    auto n64_before = [&](int k) { return k == 0 ? 0 : 1 + 3 * (k - 1); };            // 64-bit outputs before k
+    auto n64_before = [&](int k) { return k == 0 ? 0 : 1 + kPer * (k - 1); };         // 64-bit outputs before k
     auto fresh_before = [&](int q) { return h0 == 0 ? (q + 1) / 2 : q / 2; };         // outputs used by requests < q
     auto base_of = [&](int k) { return fresh_before(q_before(k)) + n64_before(k); };  // outputs before vehicle k
     if (do_reset && active && simple_geometry) {
         const int k = i;
         const bool has32 = k == 0 ? ego32 : n32;
-        Pcg64 g = pcg_at(g0, base_of(k));
+        Pcg64 g = jump(g0, base_of(k));
         uint32_t r32 = 0;
         if (has32) {
             const int rq = q_before(k);
@@ -823,7 +890,7 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
                 r32 = g0.u32;                // the half buffered before this reset
             } else {
                 // high half of the output the previous requester opened: vehicle k-1
-                Pcg64 gp = pcg_at(g0, base_of(k - 1));
+                Pcg64 gp = jump(g0, base_of(k - 1));
                 r32 = (uint32_t)(gp.next64() >> 32);
             }
             // Lemire (random_bounded_uint64, rng = L-1): rejection => serial fallback
@@ -841,6 +908,9 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
         double default_spacing = 12 + 1.0 * speed;
         double offset = spacing * default_spacing * P.spawn_exp;
         incr = offset * g.uniform(0.9, 1.1);
+        if constexpr (LINEAR) {
+            if (!is_ego) draw_linear_params(g, *T, lin);
+        }
         if (!is_ego) delta = g.uniform(P.delta_lo, P.delta_hi);
         sm.sp_x[k] = is_ego ? 3 * offset + incr : incr;  // x0 = 3 * offset; x0 += offset * U
     }
@@ -855,14 +925,14 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
             }
             // stream position after the reset
             const int Q = ego32 + (V - 1) * n32;
-            Pcg64 ge = pcg_at(g0, fresh_before(Q) + n64_before(V));
+            Pcg64 ge = jump(g0, fresh_before(Q) + n64_before(V));
             uint32_t has_f = (uint32_t)((h0 + Q) & 1), u_f = g0.u32;
             if (Q > 0) {
                 int rf = Q - 1;  // last fresh request
                 if (((h0 + rf) & 1) != 0) rf -= 1;
                 if (rf >= 0) {
                     int kf = ego32 ? rf : rf + 1;  // vehicle issuing request rf
-                    Pcg64 gp = pcg_at(g0, base_of(kf));
+                    Pcg64 gp = jump(g0, base_of(kf));
                     u_f = (uint32_t)(gp.next64() >> 32);
                 }
             }
@@ -898,6 +968,11 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
             double py = (Lv.start_y + x0 * Lv.dir_y) + 0.0 * Lv.lat_y;
             pos[base + v] = make_double2(px, py);
             hs[base + v] = make_double2(Lv.heading, sp);
+            if constexpr (LINEAR) {
+                double p[HWY_LINEAR_PARAMS] = {0.0, 0.0, 0.0, 0.0, 0.0};
+                if (!is_ego) draw_linear_params(g, *T, p);
+                for (int k = 0; k < HWY_LINEAR_PARAMS; ++k) T->params[(base + v) * HWY_LINEAR_PARAMS + k] = p[k];
+            }
             S.delta[base + v] = is_ego ? 4.0 : g.uniform(P.delta_lo, P.delta_hi);
         }
         S.rng[0 * n + e] = g.s_hi;
@@ -922,6 +997,10 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
             px = (Ln.start_x + x0 * Ln.dir_x) + 0.0 * Ln.lat_x;  // lane.position(x0, 0)
             py = (Ln.start_y + x0 * Ln.dir_y) + 0.0 * Ln.lat_y;
             heading = Ln.heading;
+            if constexpr (LINEAR) {  // (the serial path stored them itself)
+                const size_t slot = (size_t)e * S.vp + i;
+                for (int k = 0; k < HWY_LINEAR_PARAMS; ++k) T->params[slot * HWY_LINEAR_PARAMS + k] = lin[k];
+            }
         }
         int lane = closest_lane(P, px, py, heading);  // RoadObject.__init__ objects.py:46-50
         double target_speed = speed;                   // `target_speed or self.speed`
@@ -973,6 +1052,11 @@ constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full regis
 // projections in lane_distance / closest_lane, F.slow for unaligned lanes) are compiled out.  The per-substep loop
 // of this kernel is about as large as the SM's instruction cache, so code bytes on the hot path are a first-order
 // cost.
+//
+// The kernel body (hwy_highway_step.cuh) is compiled twice: highway_step_kernel (IDMVehicle traffic, LINEAR = false)
+// and highway_linear_step_kernel (LinearVehicle traffic, LINEAR = true, `T` its parameters; the block's LinearShared
+// staging follows its EnvShared array in dynamic shared memory).  Only `if constexpr (LINEAR)` branches differ, and
+// each kernel keeps the body in its own scope (an inlined device function changes the IDM kernel's code schedule).
 template <int TPE, bool AL>
 __global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
 highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
@@ -981,407 +1065,23 @@ highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighway
                     uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
                     double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
                     const int autoreset, float* __restrict__ final_obs) {
-    constexpr int NW = TPE / 32;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    EnvShared<TPE>* smem = reinterpret_cast<EnvShared<TPE>*>(smem_raw);
-    const int EPB = blockDim.x / TPE;
-    const int sub = threadIdx.x / TPE;
-    const int i = threadIdx.x % TPE;
-    const int env = blockIdx.x * EPB + sub;
-    const bool env_ok = env < S.n_envs;  // surplus envs of the last block mirror the last env
-    const int e = env_ok ? env : S.n_envs - 1;
-    EnvShared<TPE>& sm = smem[sub];
-    const int V = P.n_vehicles;
-    const bool active = i < V;
-    const size_t slot = (size_t)e * S.vp + (active ? i : 0);
-    const bool aligned = AL || lanes_aligned(P);
-    const bool congruent = AL || lanes_congruent(P);
+    constexpr bool LINEAR = false;
+    const HwyLinearTraffic* T = nullptr;
+#include "hwy_highway_step.cuh"
+}
 
-    VehicleRegs r;
-    load_vehicle(S, slot, r);
-    const int kind = meta_kind(r.meta);
-    int speed_index = (i == 0) ? S.speed_index[e] : 0;
-    double act_steer = 0.0, act_accel = 0.0;
-    // autoreset < 0 (hwy_highway_substeps): -autoreset times Road.act() + Road.step(dt) and nothing else — no
-    // action_type.act, no observation / reward / clock; the controlled vehicle acts like ControlledVehicle.act(None)
-    const int substeps_only = autoreset < 0 ? -autoreset : 0;
-    const int frames = substeps_only ? substeps_only : P.simulation_frequency / P.policy_frequency;
-    const double dt = 1.0 / P.simulation_frequency;
-
-    // ---- static masks
-    {
-        uint32_t b_cc = __ballot_sync(0xffffffffu, active && (r.meta & HWY_META_CHECK_COLLISIONS));
-        uint32_t b_ctrl = __ballot_sync(0xffffffffu, active && kind != HWY_KIND_VEHICLE);
-        if ((i & 31) == 0) {
-            sm.cc[i >> 5] = b_cc;
-            sm.ctrl[i >> 5] = b_ctrl;
-            sm.mid[i >> 5] = 0;
-        }
-        sm.last_will[i] = -1;
-        sm.crash_hit[i] = 0;
-        if (i < NW) sm.ok_left[i] = sm.ok_right[i] = 0;
-        if (i == 0) sm.n_items = 0;
-        if (active) sm.delta[i] = r.delta;
-    }
-    const IdmK K = make_idm(P);
-    // all-pairs gate (every vehicle checks collisions): rank-pruned sweep; a single checking vehicle (highway-fast)
-    // already costs one pre-check per thread
-    const bool pruned = P.others_check_collisions != 0;
-    int p = 1;
-    PHASE_INIT();
-    PHASE_MARK(0);  // load + static masks
-
-    // One iteration = stage the current state, derive its masks (+ the collision sweep of the
-    // substep that produced it), then — except after the last substep — act and integrate.
-    for (int frame = 0;; ++frame) {
-        p ^= 1;
-        Frame<TPE>& F = sm.f[p];
-        publish(P, F, i, active, r);
-        PHASE_MARK(1);  // publish
-        env_sync<TPE>();
-        PHASE_MARK(2);  // barrier after publish
-        if (i < NW) sm.mid[i] = sm.ok_left[i] = sm.ok_right[i] = 0;  // all readers are past phase B
-        if (i == 0) sm.n_items = 0;
-        // frame 0: masks only — the sweep of the stored state ran at the end of the substep that
-        // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).
-        build_frame(P, sm, F, i, active, aligned, r, dt, frame > 0, pruned, frame > 0 ? &sm.f[p ^ 1] : nullptr);
-        PHASE_MARK(3);  // ranks, masks, sweep pass 1
-        if (pruned && frame > 0) {  // uniform over the grid
-            env_sync_phase<TPE, 3>();
-            sweep_pruned(sm, F, V, i, active, dt);
-        }
-        env_sync_phase<TPE, 3>();
-        PHASE_MARK(4);  // barrier after build
-        if (active && frame > 0) apply_collisions(sm, F, i, r, dt);
-        PHASE_MARK(5);  // sweep pass 2
-        if (frame == frames) break;
-
-        // ---- action_type.act(action) on the first frame (abstract.py:294-304)
-        if (frame == 0) {
-            if (i == 0) {
-                if (kind == HWY_KIND_MDP) {
-                    // MDPVehicle.act (controller.py:295-315) + ControlledVehicle.act lane part
-                    // (:99-124); labels action.py:204.  follow_road (:135-143) cannot change the
-                    // target on the single-road highway graph (next_lane hits KeyError,
-                    // road/road.py:129-130).
-                    int a = substeps_only ? 1 : action_i[e];  // substeps only: act(None) = IDLE
-                    if (a == 3 || a == 4) {
-                        int idx = speed_to_index(P, r.speed) + (a == 3 ? 1 : -1);
-                        idx = max(0, min(idx, P.n_target_speeds - 1));
-                        speed_index = idx;
-                        r.target_speed = P.target_speeds[idx];
-                        F.ts[0] = r.target_speed;
-                    } else if (a == 0 || a == 2) {
-                        int old = meta_target(r.meta);
-                        int id = old + (a == 2 ? 1 : -1);
-                        id = max(0, min(id, P.lanes_count - 1));
-                        if (lane_reachable(P.lanes[id], r.x, r.y)) {
-                            r.meta = meta_set_target(r.meta, id);
-                            F.tgt[0] = (unsigned char)id;
-                            F.tm[old][0] &= ~1u;
-                            F.tm[id][0] |= 1u;
-                        }
-                    }
-                } else {
-                    // ContinuousAction.get_action/act (action.py:136-162): Box is float32 and
-                    // lmap (utils.py:31-33) stays in float32 (NEP 50 weak python scalars)
-                    // (substeps only: the vehicle's current action dict, or the default {0, 0} when none is given —
-                    // lmap(0) of the symmetric default ranges)
-                    float a0 = action_f ? action_f[2 * (size_t)e] : 0.0f, a1 = action_f ? action_f[2 * (size_t)e + 1] : 0.0f;
-                    if (P.act_clip) {
-                        a0 = fminf(fmaxf(a0, -1.0f), 1.0f);
-                        a1 = fminf(fmaxf(a1, -1.0f), 1.0f);
-                    }
-                    float acc = __fadd_rn((float)P.acc_lo,
-                                          __fdiv_rn(__fmul_rn(__fsub_rn(a0, -1.0f),
-                                                              (float)(P.acc_hi - P.acc_lo)), 2.0f));
-                    float st = __fadd_rn((float)P.steer_lo,
-                                         __fdiv_rn(__fmul_rn(__fsub_rn(a1, -1.0f),
-                                                             (float)(P.steer_hi - P.steer_lo)), 2.0f));
-                    act_accel = (double)acc;
-                    act_steer = (double)st;
-                }
-            }
-            env_sync<TPE>();
-        }
-
-        PHASE_MARK(6);  // ego action (+ barrier on frame 0)
-        // ---- Road.act() (road/road.py:464-467), phase A1: own-lane IDM; lane-change policy set-up
-        const int lane = meta_lane(r.meta);
-        const int tgt0 = meta_target(r.meta);
-        const bool crashed = (r.meta & HWY_META_CRASHED) != 0;
-        const bool idm_active = active && kind == HWY_KIND_IDM && !crashed;  // behavior.py:102-103
-        bool is_mid = false, fired = false;
-        double acc = 0.0, free_i = 0.0;
-        if (idm_active) {
-            free_i = idm_free_term(K.comfort_acc_max, r.speed, r.target_speed, P.lanes[lane].speed_limit, r.delta);
-            int f_own, r_own;
-            neighbours(P, F, V, lane, i, f_own, r_own);
-            acc = free_i;  // behavior.py:115-120
-            if (f_own >= 0) acc -= idm_gap_term(P, K, F, aligned, i, f_own);
-            if (lane != tgt0) {
-                // change_lane_policy, ongoing change (behavior.py:229-244).  Only a controlled
-                // vehicle v that is not on our target lane T and whose target is T when we act
-                // can abort us: candidates = (target is T now) or (may switch to T this act).
-                is_mid = true;
-                uint32_t g[NW];
-#pragma unroll
-                for (int w = 0; w < NW; ++w) {
-                    uint32_t may = F.tm[tgt0][w];
-                    uint32_t adj = (tgt0 > 0 ? F.lane_is[tgt0 - 1][w] : 0u) |
-                                   (tgt0 < P.lanes_count - 1 ? F.lane_is[tgt0 + 1][w] : 0u);
-                    may |= F.fired[w] & adj;
-                    uint32_t cand = may & sm.ctrl[w] & ~F.lane_is[tgt0][w];
-                    if (w == (i >> 5)) cand &= ~(1u << (i & 31));
-                    g[w] = 0;
-                    while (cand) {
-                        int b = __ffs(cand) - 1;
-                        cand &= cand - 1;
-                        int v = w * 32 + b;
-                        double d = lane_distance(P, F, aligned, i, v);
-                        double d_star = desired_gap(K, F, i, v);
-                        if (0 < d && d < d_star) g[w] |= 1u << b;
-                    }
-                    sm.geo[i][w] = g[w];
-                }
-                atomicOr(&sm.mid[i >> 5], 1u << (i & 31));
-            } else if (P.lane_change_delay < r.timer) {  // utils.do_every (utils.py:27-28)
-                r.timer = 0.0;
-                fired = true;
-                // side_lanes (road/road.py:200-211): id-1 then id+1.  Each admissible candidate
-                // becomes a work item; mobil() itself runs in phase A2 on a dense set of threads.
-                sm.free_t[i] = free_i;
-                sm.acc_own[i] = acc;
-                sm.f_own[i] = (signed char)f_own;
-                sm.r_own[i] = (signed char)r_own;
-                if (!(fabs(r.speed) < 1)) {
-                    for (int k = 0; k < 2; ++k) {
-                        int cand = k == 0 ? lane - 1 : lane + 1;
-                        if (cand < 0 || cand > P.lanes_count - 1) continue;
-                        if (!lane_reachable(P.lanes[cand], r.x, r.y)) continue;
-                        int slot_ = atomicAdd(&sm.n_items, 1);
-                        sm.items[slot_] = (unsigned short)(i | (cand << 8) | (k << 15));
-                    }
-                }
-            }
-        }
-        PHASE_MARK(7);  // phase A1
-        env_sync_phase<TPE, 2>();
-        PHASE_MARK(8);  // barrier after phase A1
-
-        // ---- phase A2: mobil(lane_index) (behavior.py:265-324; route None => acceleration-gain
-        // branch) for the queued (vehicle, candidate) items, one item per thread.
-        for (int t = i; t < sm.n_items; t += TPE) {
-            const int it = sm.items[t];
-            const int v = it & 0xff, cand = (it >> 8) & 0x7f, right = it >> 15;
-            const double delta_v = sm.delta[v];
-            int new_preceding, new_following;
-            neighbours_cold(P, F, V, cand, v, new_preceding, new_following);
-            double new_following_pred_a = idm_acceleration_of(P, K, F, aligned, delta_v, new_following, v);
-            if (new_following_pred_a < -P.lane_change_max_braking_imposed) continue;
-            double self_pred_a = sm.free_t[v];
-            if (new_preceding >= 0) self_pred_a -= idm_gap_term(P, K, F, aligned, v, new_preceding);
-            double self_a = sm.acc_own[v];  // acceleration(self, old_preceding)
-            double jerk = self_pred_a - self_a;
-            if (P.politeness != 0.0) {
-                const int f_o = sm.f_own[v], r_o = sm.r_own[v];
-                double new_following_a =
-                    idm_acceleration_of(P, K, F, aligned, delta_v, new_following, new_preceding);
-                double old_following_a = idm_acceleration_of(P, K, F, aligned, delta_v, r_o, v);
-                double old_following_pred_a = idm_acceleration_of(P, K, F, aligned, delta_v, r_o, f_o);
-                jerk = self_pred_a - self_a +
-                       P.politeness * (new_following_pred_a - new_following_a + old_following_pred_a -
-                                       old_following_a);
-            }
-            if (jerk < P.lane_change_min_acc_gain) continue;
-            atomicOr(right ? &sm.ok_right[v >> 5] : &sm.ok_left[v >> 5], 1u << (v & 31));
-        }
-        PHASE_MARK(13);  // phase A2
-        env_sync_phase<TPE, 2>();
-        PHASE_MARK(14);  // barrier after phase A2
-
-        // ---- Road.act() phase B (steering + target-lane IDM with the final target), then
-        // Road.step(dt): Vehicle.step (kinematics.py:130-177; IDMVehicle.step behavior.py:139-148).
-        // The new state goes to the other frame, so no barrier is needed before staging it.
-        if (active) {
-            // both side lanes may pass mobil(); the later one (id+1) wins (behavior.py:252-263)
-            int tgt = tgt0;
-            if (fired) {
-                if (test_bit(sm.ok_right, i))
-                    tgt = lane + 1;
-                else if (test_bit(sm.ok_left, i))
-                    tgt = lane - 1;
-            }
-            if (is_mid) {
-                // Ordered resolution of the Gauss-Seidel abort scan (behavior.py:229-244).  Vehicles
-                // act in list order: vehicle j sees the NEW target of every earlier vehicle and the
-                // OLD one of every later vehicle.  Only events on our target lane T matter (a
-                // vehicle leaving T, or an aborting vehicle returning to its own lane, sits ON the
-                // lane it now targets and is excluded by `lane_index != T`), so each mid-change
-                // vehicle replays, redundantly and in registers, the decisions of the earlier
-                // mid-change vehicles that share its target.
-                const int T = tgt0, iw = i >> 5, ib = i & 31;
-                uint32_t tmT[NW], lneT[NW], chgT[NW], ab[NW];
-#pragma unroll
-                for (int w = 0; w < NW; ++w) {
-                    tmT[w] = F.tm[T][w];
-                    lneT[w] = ~F.lane_is[T][w];
-                    // vehicles whose MOBIL decision just switched their target to T
-                    chgT[w] = (T > 0 ? sm.ok_right[w] & F.lane_is[T - 1][w] : 0u) |
-                              (T < P.lanes_count - 1 ? sm.ok_left[w] & ~sm.ok_right[w] & F.lane_is[T + 1][w] : 0u);
-                    ab[w] = 0;
-                }
-#pragma unroll
-                for (int w = 0; w < NW; ++w) {
-                    uint32_t m = sm.mid[w] & tmT[w];
-                    if (w > iw) m = 0;
-                    if (w == iw) m &= (2u << ib) - 1u;  // mids up to and including ourselves
-                    while (m) {
-                        int b = __ffs(m) - 1;
-                        m &= m - 1;
-                        int j = w * 32 + b;
-                        uint32_t hit = 0;
-#pragma unroll
-                        for (int w2 = 0; w2 < NW; ++w2) {
-                            uint32_t below = w2 < w ? ~0u : (w2 == w ? (1u << b) - 1u : 0u);
-                            uint32_t cur = (tmT[w2] & ~ab[w2]) | (chgT[w2] & below);
-                            hit |= sm.geo[j][w2] & lneT[w2] & cur;
-                        }
-                        if (hit) ab[w] |= 1u << b;  // behavior.py:241-243: target := current lane
-                    }
-                }
-                if ((ab[iw] >> ib) & 1u) tgt = lane;
-            }
-            // IDMVehicle.act (behavior.py:109-112) and ControlledVehicle.act(None)
-            // (controller.py:126-133, runs even when crashed) share the steering law
-            double sin_beta = 0.0, cos_beta = 1.0;  // crashed: steering 0 (clip_actions :155-158)
-            if (idm_active || (kind == HWY_KIND_MDP && !crashed)) {
-                double xs = steering_sin_slip(P.lanes[tgt], r.x, r.y, r.heading, r.speed);
-                beta_of_controlled(xs, sin_beta, cos_beta);
-            } else if (kind == HWY_KIND_VEHICLE && !crashed) {
-                beta_of_angle(act_steer, sin_beta, cos_beta);
-            }
-            if (idm_active) {
-                if (lane != tgt) {  // behavior.py:121-131
-                    int f_t, r_t;
-                    neighbours_cold(P, F, V, tgt, i, f_t, r_t);
-                    double tacc = free_i;
-                    if (f_t >= 0) tacc -= idm_gap_term(P, K, F, aligned, i, f_t);
-                    acc = fmin(acc, tacc);
-                }
-                act_accel = clipd(acc, -P.acc_max, P.acc_max);
-            } else if (kind == HWY_KIND_MDP) {
-                act_accel = kKpA * (r.target_speed - r.speed);  // speed_control :189-198
-            }
-            r.meta = meta_set_target(r.meta, tgt);
-
-            PHASE_MARK(9);  // phase B
-            if (kind == HWY_KIND_IDM) r.timer += dt;
-            if (crashed) {  // clip_actions :155-168
-                act_steer = 0.0;
-                act_accel = -1.0 * r.speed;
-            }
-            if (r.speed > kMaxSpeed)
-                act_accel = fmin(act_accel, 1.0 * (kMaxSpeed - r.speed));
-            else if (r.speed < kMinSpeed)
-                act_accel = fmax(act_accel, 1.0 * (kMinSpeed - r.speed));
-            // cos/sin(heading + beta) by angle addition from the staged cos/sin(heading)
-            const double ch = F.c[i], sh = F.s[i];
-            double cs = ch * cos_beta - sh * sin_beta, sn = sh * cos_beta + ch * sin_beta;
-            double vx = r.speed * cs, vy = r.speed * sn;
-            r.x += vx * dt;
-            r.y += vy * dt;
-            if (r.meta & HWY_META_HAS_IMPACT) {
-                r.x += r.imp_x;
-                r.y += r.imp_y;
-                r.meta = (r.meta | HWY_META_CRASHED) & ~HWY_META_HAS_IMPACT;
-            }
-            r.heading += div_finite(r.speed * sin_beta, kVehLength / 2) * dt;
-            r.speed += act_accel * dt;
-            int nl = closest_lane(P, r.x, r.y, r.heading, congruent);  // on_state_update :170-177
-            r.meta = meta_set_lane(r.meta, nl);
-            if (kind == HWY_KIND_VEHICLE) r.meta = meta_set_target(r.meta, nl);  // schema: mirrors lane
-        }
-        PHASE_MARK(10);  // integrate
-    }
-
-    PHASE_MARK(11);
-    if (substeps_only) {  // uniform over the grid
-        if (active && env_ok) store_vehicle(S, slot, r);
-        return;
-    }
-    // ---- epilogue: state back to HBM, observation, reward, termination
-    const Frame<TPE>& F = sm.f[p];
-    const size_t obs_off = (size_t)e * P.obs_vehicles_count * obs_columns(P);
-    float* obs_env = obs + obs_off;
-    kinematics_observe(P, F, sm.key, i, r.heading, env_ok ? obs_env : nullptr,
-                       (autoreset && final_obs) ? final_obs + obs_off : nullptr);
-    if (i == 0) {
-        sm.done = 0;
-        sm.sp_fallback = 0;
-    }
-    if (i == 0 && env_ok) {
-        // envs/highway_env.py:100-151
-        const int lane = meta_lane(r.meta);
-        const HwyStraightLane& L = P.lanes[lane];
-        int rl = kind == HWY_KIND_VEHICLE ? lane : meta_target(r.meta);
-        double forward_speed = r.speed * F.c[0];
-        double scaled_speed = lmap(forward_speed, P.reward_speed_lo, P.reward_speed_hi, 0.0, 1.0);
-        double es, elat;
-        lane_local(L, r.x, r.y, es, elat);
-        bool on_road = lane_on(L, es, elat, 0.0);
-        bool is_crashed = (r.meta & HWY_META_CRASHED) != 0;
-        int nl1 = P.lanes_count - 1 > 1 ? P.lanes_count - 1 : 1;
-        double rew = 0.0;
-        rew = rew + P.collision_reward * (is_crashed ? 1.0 : 0.0);
-        rew = rew + P.right_lane_reward * ((double)rl / (double)nl1);
-        rew = rew + P.high_speed_reward * clipd(scaled_speed, 0.0, 1.0);
-        rew = rew + 0.0 * (on_road ? 1.0 : 0.0);
-        if (P.normalize_reward)
-            rew = lmap(rew, P.collision_reward, P.high_speed_reward + P.right_lane_reward, 0.0, 1.0);
-        rew *= on_road ? 1.0 : 0.0;
-        double t = S.time[e] + 1.0 / P.policy_frequency;  // abstract.py:274
-        S.time[e] = t;
-        S.speed_index[e] = speed_index;
-        reward[e] = rew;
-        terminated[e] = (uint8_t)(is_crashed || (P.offroad_terminal && !on_road));
-        truncated[e] = (uint8_t)(t >= P.duration);
-        if (info_speed) info_speed[e] = r.speed;  // abstract.py:200-217 _info
-        if (info_crashed) info_crashed[e] = (uint8_t)is_crashed;
-        if (S.reward_terms) {  // _rewards (highway_env.py:118-137): info["rewards"]
-            double* rt = S.reward_terms + (size_t)e * HWY_REWARD_TERMS;
-            rt[0] = is_crashed ? 1.0 : 0.0;
-            rt[1] = (double)rl / (double)nl1;
-            rt[2] = clipd(scaled_speed, 0.0, 1.0);
-            rt[3] = on_road ? 1.0 : 0.0;
-            rt[4] = 0.0;
-        }
-        sm.done = autoreset && (is_crashed || (P.offroad_terminal && !on_road) || t >= P.duration);
-    }
-    if (autoreset) {
-        // ---- SameStep autoreset fused into the step: envs that ended re-spawn from their own
-        // numpy stream and return the reset observation (gymnasium AutoresetMode.SAME_STEP)
-        env_sync<TPE>();
-        const bool do_reset = env_ok && sm.done;
-        const bool simple_geometry = aligned && P.lanes[0].start_x == 0.0 && P.lanes[0].dir_x == 1.0;
-        spawn_fused(P, S, sm, e, i, active, do_reset, simple_geometry, r, speed_index);
-        Frame<TPE>& G = sm.f[p ^ 1];
-        if (do_reset) publish(P, G, i, active, r);
-        // barrier + "does any env of this block re-spawn?": the second observation runs under a block-uniform
-        // condition, so that all threads of the block meet the same barrier instructions (a per-env condition around
-        // __syncthreads() is what compute-sanitizer's synccheck rejects, even though the arrival counts match)
-        const bool any_reset = __syncthreads_or(do_reset) != 0;
-        if (any_reset) {
-            kinematics_observe(P, G, sm.key, i, r.heading, do_reset ? obs_env : nullptr);
-            if (do_reset && i == 0) {
-                S.time[e] = 0.0;
-                S.speed_index[e] = speed_index;
-            }
-        }
-    }
-    if (active && env_ok) store_vehicle(S, slot, r);
-    if (autoreset && active && env_ok && sm.done) S.delta[slot] = r.delta;
-    PHASE_MARK(12);  // epilogue
+// LinearVehicle / AggressiveVehicle / DefensiveVehicle traffic (vehicle/behavior.py:350-583)
+template <int TPE, bool AL>
+__global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
+highway_linear_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
+                           const __grid_constant__ HwyLinearTraffic T_, const int32_t* __restrict__ action_i,
+                           const float* __restrict__ action_f, float* __restrict__ obs, double* __restrict__ reward,
+                           uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
+                           double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
+                           const int autoreset, float* __restrict__ final_obs) {
+    constexpr bool LINEAR = true;
+    const HwyLinearTraffic* T = &T_;
+#include "hwy_highway_step.cuh"
 }
 
 // ------------------------------------------------------------------ observe-only kernel
@@ -1418,97 +1118,23 @@ highway_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHigh
 // Vehicle.create_random (vehicle/kinematics.py:50-104), IDMVehicle.__init__ timer and
 // randomize_behavior (behavior.py:64-69), MDPVehicle.__init__ (controller.py:284-293).
 // The spawn is a sequential chain on the env's PCG64 stream => one thread per env.
+// LINEAR: LinearVehicle.randomize_behavior (behavior.py:406-415) draws the traffic's parameters into T->params.
 __global__ void __launch_bounds__(128)
 highway_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                      const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b,
                      int use_mask) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if (use_mask && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
-    const int n = S.n_envs;
-    Pcg64 g;
-    g.s_hi = S.rng[0 * (size_t)n + e];
-    g.s_lo = S.rng[1 * (size_t)n + e];
-    g.i_hi = S.rng[2 * (size_t)n + e];
-    g.i_lo = S.rng[3 * (size_t)n + e];
-    u64 w4 = S.rng[4 * (size_t)n + e];
-    g.has32 = (uint32_t)(w4 >> 32);
-    g.u32 = (uint32_t)w4;
+    constexpr bool LINEAR = false;
+    const HwyLinearTraffic* T = nullptr;
+#include "hwy_highway_reset.cuh"
+}
 
-    double x_max = 0.0;  // running max of the longitudinal coordinates of spawned vehicles
-    bool aligned = true;  // all lanes share origin-x and direction => s is lane independent
-    for (int l = 1; l < P.lanes_count; ++l)
-        aligned = aligned && P.lanes[l].start_x == P.lanes[0].start_x &&
-                        P.lanes[l].dir_x == P.lanes[0].dir_x && P.lanes[l].dir_y == 0.0 &&
-                        P.lanes[0].dir_y == 0.0;
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
-    const size_t base = (size_t)e * S.vp;
-    int ego_speed_index = -1;
-    for (int v = 0; v < P.n_vehicles; ++v) {
-        const bool is_ego = v == 0;
-        // choice(list(graph.keys())) / choice(list(graph[_from].keys())): single element => no draw
-        int id = (is_ego && P.initial_lane_id >= 0) ? P.initial_lane_id : g.choice(P.lanes_count);
-        const HwyStraightLane& L = P.lanes[id];
-        double speed = is_ego ? P.ego_speed : g.uniform(0.7 * L.speed_limit, 0.8 * L.speed_limit);
-        double spacing = is_ego ? P.ego_spacing : 1 / P.vehicles_density;
-        double default_spacing = 12 + 1.0 * speed;
-        double offset = spacing * default_spacing * P.spawn_exp;
-        double x0;
-        if (v > 0) {
-            if (aligned) {
-                x0 = x_max;
-            } else {  // np.max over lane.local_coordinates(v.position)[0] on the chosen lane
-                x0 = lane_s(L, pos[base].x, pos[base].y);
-                for (int j = 1; j < v; ++j) x0 = fmax(x0, lane_s(L, pos[base + j].x, pos[base + j].y));
-            }
-        } else {
-            x0 = 3 * offset;
-        }
-        x0 += offset * g.uniform(0.9, 1.1);
-        // lane.position(x0, 0), lane.heading_at(x0)  (road/lane.py:192-200)
-        double px = (L.start_x + x0 * L.dir_x) + 0.0 * L.lat_x;
-        double py = (L.start_y + x0 * L.dir_y) + 0.0 * L.lat_y;
-        double heading = L.heading;
-        double s_here = lane_s(L, px, py);
-        x_max = v == 0 ? s_here : fmax(x_max, s_here);
-        int lane = closest_lane(P, px, py, heading);  // RoadObject.__init__ objects.py:46-50
-        double target_speed = speed;                   // `target_speed or self.speed`
-        double timer = 0.0, delta = 4.0;
-        int kind, cc;
-        if (is_ego) {
-            cc = 1;
-            if (P.action_type == 0) {
-                kind = HWY_KIND_MDP;
-                ego_speed_index = speed_to_index(P, target_speed);
-                target_speed = P.target_speeds[ego_speed_index];
-            } else {
-                kind = HWY_KIND_VEHICLE;
-            }
-        } else {
-            kind = HWY_KIND_IDM;
-            cc = P.others_check_collisions;
-            timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
-            delta = g.uniform(P.delta_lo, P.delta_hi);                 // behavior.py:66-69
-        }
-        pos[base + v] = make_double2(px, py);
-        hs[base + v] = make_double2(heading, speed);
-        tt[base + v] = make_double2(target_speed, timer);
-        imp[base + v] = make_double2(0.0, 0.0);
-        S.delta[base + v] = delta;
-        S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) |
-                           (cc ? HWY_META_CHECK_COLLISIONS : 0) | (kind << HWY_META_KIND_SHIFT) |
-                           HWY_META_PRESENT;
-    }
-    S.speed_index[e] = ego_speed_index;
-    S.time[e] = 0.0;
-    S.rng[0 * (size_t)n + e] = g.s_hi;
-    S.rng[1 * (size_t)n + e] = g.s_lo;
-    S.rng[2 * (size_t)n + e] = g.i_hi;
-    S.rng[3 * (size_t)n + e] = g.i_lo;
-    S.rng[4 * (size_t)n + e] = ((u64)g.has32 << 32) | g.u32;
+__global__ void __launch_bounds__(128)
+highway_linear_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
+                            const __grid_constant__ HwyLinearTraffic T_, const uint8_t* __restrict__ mask_a,
+                            const uint8_t* __restrict__ mask_b, int use_mask) {
+    constexpr bool LINEAR = true;
+    const HwyLinearTraffic* T = &T_;
+#include "hwy_highway_reset.cuh"
 }
 
 // ------------------------------------------------------------------ test entries
@@ -1734,26 +1360,34 @@ bool lanes_congruent_host(const HwyHighwayParams* p) {
     return ok;
 }
 
+// t == nullptr: IDMVehicle traffic (highway_step_kernel); else LinearVehicle traffic (highway_linear_step_kernel)
 template <int TPE, bool AL>
-int launch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                const float* action_f, float* obs, double* reward, uint8_t* terminated,
+int launch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
                 uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset,
                 float* final_obs, int blocks, int epb, cudaStream_t st) {
     if (autoreset > 0 && ensure_pcg_jump(st)) return 1;
-    size_t smem = (size_t)epb * sizeof(hwy::EnvShared<TPE>);
+    size_t smem = (size_t)epb * (sizeof(hwy::EnvShared<TPE>) + (t ? sizeof(hwy::LinearShared<TPE>) : 0));
     // the attribute is per device (and per template instance): cache it by device ordinal
-    static std::atomic<size_t> configured[64];
+    static std::atomic<size_t> configured[2][64];
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
-    if (smem > configured[dev].load(std::memory_order_relaxed)) {
-        cudaError_t err = cudaFuncSetAttribute(hwy::highway_step_kernel<TPE, AL>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (smem > configured[t != nullptr][dev].load(std::memory_order_relaxed)) {
+        cudaError_t err = t ? cudaFuncSetAttribute(hwy::highway_linear_step_kernel<TPE, AL>,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                            : cudaFuncSetAttribute(hwy::highway_step_kernel<TPE, AL>,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-        configured[dev].store(smem, std::memory_order_relaxed);
+        configured[t != nullptr][dev].store(smem, std::memory_order_relaxed);
     }
-    hwy::highway_step_kernel<TPE, AL><<<blocks, TPE * epb, smem, st>>>(
-        *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-        autoreset, final_obs);
+    if (t)
+        hwy::highway_linear_step_kernel<TPE, AL><<<blocks, TPE * epb, smem, st>>>(
+            *p, *s, *t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+            autoreset, final_obs);
+    else
+        hwy::highway_step_kernel<TPE, AL><<<blocks, TPE * epb, smem, st>>>(
+            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+            autoreset, final_obs);
     return 0;
 }
 
@@ -1776,12 +1410,28 @@ int launch_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const uint
     hwy::highway_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, mask_a, mask_b, use_mask);
     return check_launch("highway_reset_kernel");
 }
+
+int launch_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                        const uint8_t* mask_a, const uint8_t* mask_b, int use_mask, cudaStream_t st) {
+    int blocks = (s->n_envs + 127) / 128;
+    hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b, use_mask);
+    return check_launch("highway_linear_reset_kernel");
+}
+
+int validate_linear(const HwyLinearTraffic* t) {
+    if (!t || !t->params) return fail("%s", "null linear traffic parameters");
+    return 0;
+}
 }  // namespace
 
 namespace {
-int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i, const float* action_f,
-                  float* obs, double* reward, uint8_t* terminated, uint8_t* truncated, double* info_speed,
-                  uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st);
+int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                  const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
+                  uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
+                  cudaStream_t st);
+int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                    const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                    int autoreset);
 }
 
 extern "C" {
@@ -1862,14 +1512,9 @@ int hwy_highway_step(const HwyHighwayParams* p, const HwyHighwayState* s, const 
                      const float* action_f, float* obs, double* reward, uint8_t* terminated,
                      uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset,
                      float* final_obs, void* stream) {
-    if (validate(p, s)) return 1;
-    if (!obs || !reward || !terminated || !truncated) return fail("%s", "null output pointer");
-    if (p->action_type == 0 && !action_i) return fail("%s", "DiscreteMetaAction needs action_i");
-    if (p->action_type == 1 && !action_f) return fail("%s", "ContinuousAction needs action_f");
-    if (autoreset != HWY_AUTORESET_DISABLED && autoreset != HWY_AUTORESET_SAME_STEP)
-        return fail("%s", "unknown autoreset mode");
-    return dispatch_step(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, autoreset,
-                         final_obs, (cudaStream_t)stream);
+    if (check_step_args(p, s, action_i, action_f, obs, reward, terminated, truncated, autoreset)) return 1;
+    return dispatch_step(p, s, nullptr, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+                         autoreset, final_obs, (cudaStream_t)stream);
 }
 
 /* B4 seam of the reference (abstract.py:304-307 minus action_type.act): n_substeps x (Road.act(); Road.step(dt)). */
@@ -1877,16 +1522,68 @@ int hwy_highway_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, in
                          void* stream) {
     if (validate(p, s)) return 1;
     if (n_substeps < 1 || n_substeps > 4096) return fail("%s", "n_substeps must be in 1..4096");
-    return dispatch_step(p, s, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, -n_substeps, nullptr,
-                         (cudaStream_t)stream);
+    return dispatch_step(p, s, nullptr, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                         -n_substeps, nullptr, (cudaStream_t)stream);
+}
+
+// ---- LinearVehicle traffic: the same four entry points on the linear kernels
+int hwy_highway_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                             const uint8_t* mask, float* obs, void* stream) {
+    if (validate(p, s) || validate_linear(t)) return 1;
+    cudaStream_t st = (cudaStream_t)stream;
+    int use_mask = mask != nullptr;
+    if (ensure_pcg_jump(st)) return 1;
+    if (launch_linear_reset(p, s, t, mask, nullptr, use_mask, st)) return 1;
+    if (obs) return launch_observe(p, s, mask, nullptr, use_mask, obs, st);
+    return 0;
+}
+
+int hwy_highway_linear_autoreset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                                 const uint8_t* terminated, const uint8_t* truncated, float* obs, void* stream) {
+    if (validate(p, s) || validate_linear(t)) return 1;
+    if (!terminated || !truncated || !obs) return fail("%s", "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (launch_linear_reset(p, s, t, terminated, truncated, 1, st)) return 1;
+    return launch_observe(p, s, terminated, truncated, 1, obs, st);
+}
+
+int hwy_highway_linear_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                            const int32_t* action_i, const float* action_f, float* obs, double* reward,
+                            uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
+                            int autoreset, float* final_obs, void* stream) {
+    if (check_step_args(p, s, action_i, action_f, obs, reward, terminated, truncated, autoreset)) return 1;
+    if (validate_linear(t)) return 1;
+    return dispatch_step(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+                         autoreset, final_obs, (cudaStream_t)stream);
+}
+
+int hwy_highway_linear_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                                int n_substeps, const float* action_f, void* stream) {
+    if (validate(p, s) || validate_linear(t)) return 1;
+    if (n_substeps < 1 || n_substeps > 4096) return fail("%s", "n_substeps must be in 1..4096");
+    return dispatch_step(p, s, t, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                         -n_substeps, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"
 
 namespace {
-int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i, const float* action_f,
-                  float* obs, double* reward, uint8_t* terminated, uint8_t* truncated, double* info_speed,
-                  uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st) {
+int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                    const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                    int autoreset) {
+    if (validate(p, s)) return 1;
+    if (!obs || !reward || !terminated || !truncated) return fail("%s", "null output pointer");
+    if (p->action_type == 0 && !action_i) return fail("%s", "DiscreteMetaAction needs action_i");
+    if (p->action_type == 1 && !action_f) return fail("%s", "ContinuousAction needs action_f");
+    if (autoreset != HWY_AUTORESET_DISABLED && autoreset != HWY_AUTORESET_SAME_STEP)
+        return fail("%s", "unknown autoreset mode");
+    return 0;
+}
+
+int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                  const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
+                  uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
+                  cudaStream_t st) {
     int tpe = tpe_for(p->n_vehicles);
     int epb = step_envs_per_block(tpe, s->n_envs);
     int blocks = (s->n_envs + epb - 1) / epb;
@@ -1894,7 +1591,7 @@ int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int
     const char* force_general = getenv("HWYB200_GENERAL_LANES");
     const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
 #define HWY_LAUNCH_STEP(T, A)                                                                              \
-    launch_step<T, A>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
+    launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
                       autoreset, final_obs, blocks, epb, st)
     int rc;
     if (tpe == 32)
@@ -1905,7 +1602,7 @@ int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int
         rc = al ? HWY_LAUNCH_STEP(128, true) : HWY_LAUNCH_STEP(128, false);
 #undef HWY_LAUNCH_STEP
     if (rc) return 1;
-    if (check_launch("highway_step_kernel")) return 1;
+    if (check_launch(t ? "highway_linear_step_kernel" : "highway_step_kernel")) return 1;
     return 0;
 }
 }  // namespace

@@ -28,6 +28,27 @@ from .common.observation import KinematicObservation, observation_factory
 from .common.vector_env import BatchedVectorEnv
 from ..road.network import NetworkTable
 
+IDM_VEHICLE = "highway_env.vehicle.behavior.IDMVehicle"
+# LinearVehicle and its subclasses (vehicle/behavior.py:350-583) -> LANE_CHANGE_MIN_ACC_GAIN.  On the highway the three
+# are one model: randomize_behavior overwrites the subclasses' ACCELERATION_PARAMETERS with draws from the
+# ACCELERATION_RANGE they inherit from LinearVehicle.
+LINEAR_VEHICLE_TYPES = {
+    "highway_env.vehicle.behavior.LinearVehicle": 0.2,
+    "highway_env.vehicle.behavior.AggressiveVehicle": 1.0,
+    "highway_env.vehicle.behavior.DefensiveVehicle": 1.0,
+}
+
+
+def linear_ranges():
+    """LinearVehicle.ACCELERATION_RANGE / STEERING_RANGE (behavior.py:353-371) as (lo, hi - lo) per parameter, with
+    the reference's numpy arithmetic (KP_HEADING = 1 / TAU_HEADING, KP_LATERAL = 1 / TAU_LATERAL, controller.py:24-33)."""
+    kp_heading, kp_lateral = 1 / 0.2, 1 / 0.6
+    acc = np.array([0.3, 0.3, 2.0])
+    steer = np.array([kp_heading, kp_heading * kp_lateral])
+    acc_range = np.array([0.5 * acc, 1.5 * acc])
+    steer_range = np.array([steer - np.array([0.07, 1.5]), steer + np.array([0.07, 1.5])])
+    return acc_range[0], acc_range[1] - acc_range[0], steer_range[0], steer_range[1] - steer_range[0]
+
 
 class BatchedHighwayEnv(BatchedVectorEnv):
     """``num_envs`` independent highway roads stepped by the sm_90a kernels."""
@@ -63,8 +84,11 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         cfg = self.config
         if cfg.get("controlled_vehicles", 1) != 1:
             raise NotImplementedError("controlled_vehicles != 1 (multi-agent) is not on the accelerated path")
-        if cfg.get("other_vehicles_type") != "highway_env.vehicle.behavior.IDMVehicle":
-            raise NotImplementedError("only IDMVehicle traffic is on the accelerated path")
+        ovt = cfg.get("other_vehicles_type")
+        if ovt != IDM_VEHICLE and ovt not in LINEAR_VEHICLE_TYPES:
+            raise NotImplementedError("only IDMVehicle and LinearVehicle / AggressiveVehicle / DefensiveVehicle traffic "
+                                      "is on the accelerated path")
+        self._linear = ovt in LINEAR_VEHICLE_TYPES
         if cfg.get("neighbour_vehicles_connected_lanes"):
             raise NotImplementedError("connected-lane neighbour search (v1/v2 ids) is not implemented")
         if cfg.get("manual_control"):
@@ -99,6 +123,9 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         p.politeness, p.lane_change_min_acc_gain = 0.0, 0.2
         p.lane_change_max_braking_imposed, p.lane_change_delay = 2.0, 1.0
         p.delta_lo, p.delta_hi = 3.5, 4.5
+        if self._linear:  # LinearVehicle.TIME_WANTED (behavior.py:373) and the class's LANE_CHANGE_MIN_ACC_GAIN
+            p.time_wanted = 2.5
+            p.lane_change_min_acc_gain = LINEAR_VEHICLE_TYPES[ovt]
         p.perception_distance = self.PERCEPTION_DISTANCE
         self._fused_obs.fill_params(p)
         self.action_type.fill_params(p)
@@ -127,7 +154,7 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         K = int(self._params.obs_vehicles_count)
         F = int(self._params.obs_n_features) or 5
         plugin_shape = tuple(self.single_observation_space.shape) if self._plugin_standalone else None
-        key = (n, vp, K, F, int(self._params.action_type), plugin_shape)
+        key = (n, vp, K, F, int(self._params.action_type), plugin_shape, self._linear)
         if self._allocated_for == key:
             return
         z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=dev)  # noqa: E731
@@ -166,6 +193,15 @@ class BatchedHighwayEnv(BatchedVectorEnv):
             self._speed_index.data_ptr(), self._time.data_ptr(), self._rng.data_ptr())
         st.reward_terms = self._reward_terms.data_ptr()
         self._state = st
+        self._traffic = None
+        if self._linear:  # per-vehicle ACCELERATION_PARAMETERS (3) + STEERING_PARAMETERS (2), see HwyLinearTraffic
+            self._linear_params = z(n, vp, N.HWY_LINEAR_PARAMS, dtype=torch.float64)
+            t = N.HwyLinearTraffic()
+            t.params = self._linear_params.data_ptr()
+            acc_lo, acc_span, steer_lo, steer_span = linear_ranges()
+            t.acc_lo[:], t.acc_span[:] = [float(x) for x in acc_lo], [float(x) for x in acc_span]
+            t.steer_lo[:], t.steer_span[:] = [float(x) for x in steer_lo], [float(x) for x in steer_span]
+            self._traffic = t
         self._allocated_for = key
 
     # ------------------------------------------------------------------ family kernels
@@ -176,26 +212,34 @@ class BatchedHighwayEnv(BatchedVectorEnv):
 
     def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
         """Re-spawn the envs set in mask_a or mask_b (every env without masks) from their streams."""
+        lib, P, S = self._lib, C.byref(self._params), C.byref(self._state)
         with torch.cuda.device(self.device):
-            if mask_b is None:
-                N.check(self._lib.hwy_highway_reset(C.byref(self._params), C.byref(self._state), mask_a, obs_ptr,
-                                                    self._stream()))
+            if self._traffic is not None:
+                T = C.byref(self._traffic)
+                if mask_b is None:
+                    N.check(lib.hwy_highway_linear_reset(P, S, T, mask_a, obs_ptr, self._stream()))
+                else:
+                    N.check(lib.hwy_highway_linear_autoreset(P, S, T, mask_a, mask_b, obs_ptr, self._stream()))
+            elif mask_b is None:
+                N.check(lib.hwy_highway_reset(P, S, mask_a, obs_ptr, self._stream()))
             else:
-                N.check(self._lib.hwy_highway_autoreset(C.byref(self._params), C.byref(self._state), mask_a, mask_b,
-                                                        obs_ptr, self._stream()))
+                N.check(lib.hwy_highway_autoreset(P, S, mask_a, mask_b, obs_ptr, self._stream()))
 
     def _step_kernels(self, act) -> None:
         ai = act.data_ptr() if self._params.action_type == 0 else None
         af = act.data_ptr() if self._params.action_type == 1 else None
         # the step kernel re-spawns finished envs itself unless a standalone plugin must observe the final state first
         fused_reset = self.autoreset_mode == "SameStep" and not self._plugin_standalone
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_highway_step(
-                C.byref(self._params), C.byref(self._state), ai, af, self._fused_out.data_ptr(),
-                self._reward.data_ptr(), self._terminated.data_ptr(), self._truncated.data_ptr(),
-                self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
+        args = (ai, af, self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
+                self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
                 N.AUTORESET_SAME_STEP if fused_reset else N.AUTORESET_DISABLED,
-                self._final_obs.data_ptr() if fused_reset else None, self._stream()))
+                self._final_obs.data_ptr() if fused_reset else None, self._stream())
+        with torch.cuda.device(self.device):
+            if self._traffic is not None:
+                N.check(self._lib.hwy_highway_linear_step(C.byref(self._params), C.byref(self._state),
+                                                          C.byref(self._traffic), *args))
+            else:
+                N.check(self._lib.hwy_highway_step(C.byref(self._params), C.byref(self._state), *args))
 
     def _same_step_autoreset(self, info) -> None:
         if self._plugin_standalone:
@@ -257,8 +301,32 @@ class BatchedHighwayEnv(BatchedVectorEnv):
                 raise ValueError("pass the continuous (throttle, steering) pair, not a DiscreteAction index")
             af = self._stage_actions(action).data_ptr()
         with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_highway_substeps(C.byref(self._params), C.byref(self._state), int(n_substeps), af,
-                                                   self._stream()))
+            if self._traffic is not None:
+                N.check(self._lib.hwy_highway_linear_substeps(C.byref(self._params), C.byref(self._state),
+                                                              C.byref(self._traffic), int(n_substeps), af,
+                                                              self._stream()))
+            else:
+                N.check(self._lib.hwy_highway_substeps(C.byref(self._params), C.byref(self._state), int(n_substeps),
+                                                       af, self._stream()))
+
+    # ------------------------------------------------------------------ state import / export
+    def state_dict(self) -> dict:
+        """The base fields; with LinearVehicle traffic also every vehicle's ``acceleration_parameters`` [N, V, 3] and
+        ``steering_parameters`` [N, V, 2] (zero for the controlled vehicle)."""
+        sd = super().state_dict()
+        if self._traffic is not None:
+            lp = self._linear_params[:, :self.V].cpu().numpy()
+            sd["acceleration_parameters"] = lp[..., :3].copy()
+            sd["steering_parameters"] = lp[..., 3:].copy()
+        return sd
+
+    def load_state_dict(self, sd: dict, env_ids=None) -> None:
+        super().load_state_dict(sd, env_ids)
+        if self._traffic is not None and "acceleration_parameters" in sd:
+            idx = slice(None) if env_ids is None else torch.from_numpy(np.asarray(env_ids, dtype=np.int64)).to(self.device)
+            lp = np.concatenate([np.asarray(sd["acceleration_parameters"], dtype=np.float64),
+                                 np.asarray(sd["steering_parameters"], dtype=np.float64)], axis=-1)
+            self._linear_params[idx, :self.V] = torch.from_numpy(np.ascontiguousarray(lp)).to(self.device)
 
 
 class BatchedHighwayEnvFast(BatchedHighwayEnv):

@@ -195,6 +195,34 @@ int hwy_highway_autoreset(const HwyHighwayParams *p, const HwyHighwayState *s,
                           const uint8_t *terminated, const uint8_t *truncated, float *obs,
                           void *stream);
 
+/* LinearVehicle traffic (vehicle/behavior.py:350-583; AggressiveVehicle and DefensiveVehicle
+ * are the same model on the highway, they differ only in p->lane_change_min_acc_gain).  Every
+ * traffic vehicle keeps the parameters randomize_behavior drew for it (behavior.py:406-415):
+ *   params[5*(e*vp+v) + 0..2] = ACCELERATION_PARAMETERS, + 3..4 = STEERING_PARAMETERS
+ * (DEVICE, [n_envs*vp*5] doubles; the controlled vehicle's row is zero).  A reset draws
+ *   ACCELERATION_PARAMETERS = acc_lo + uniform(size=3) * acc_span,
+ *   STEERING_PARAMETERS     = steer_lo + uniform(size=2) * steer_span
+ * with acc_lo = ACCELERATION_RANGE[0], acc_span = ACCELERATION_RANGE[1] - ACCELERATION_RANGE[0]
+ * (likewise steering) as numpy evaluates them on the host.  p->time_wanted is the class's
+ * TIME_WANTED (2.5).  The _linear entry points are the IDM ones with this traffic model. */
+#define HWY_LINEAR_PARAMS 5
+typedef struct HwyLinearTraffic {
+    double *params;
+    double acc_lo[3], acc_span[3];
+    double steer_lo[2], steer_span[2];
+} HwyLinearTraffic;
+
+int hwy_highway_linear_reset(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                             const uint8_t *mask, float *obs, void *stream);
+int hwy_highway_linear_step(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                            const int32_t *action_i, const float *action_f, float *obs, double *reward,
+                            uint8_t *terminated, uint8_t *truncated, double *info_speed, uint8_t *info_crashed,
+                            int autoreset, float *final_obs, void *stream);
+int hwy_highway_linear_substeps(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                                int n_substeps, const float *action_f, void *stream);
+int hwy_highway_linear_autoreset(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                                 const uint8_t *terminated, const uint8_t *truncated, float *obs, void *stream);
+
 
 /* ====================================================================== general road networks
  * roundabout-v0 (envs/roundabout_env.py): Straight / Sine / Circular lanes (road/lane.py:159-384),
