@@ -1,8 +1,9 @@
 // hwy_highway.cu — sm_90a kernels + C ABI for the straight-highway family
 // (highway-v0 / highway-fast-v0) of the batched HighwayEnv hot path.
 //
-// Thread mapping: one (env, vehicle) pair per thread, TPE threads per env (32/64/128, the
-// next power of two >= n_vehicles).  The whole AbstractEnv.step — every substep of
+// Thread mapping of the step kernel: one (env, vehicle) pair per thread, each env a dense segment of V = n_vehicles
+// consecutive threads of the block (segments start anywhere in a warp); TPE (32/64/128, the next power of two >= V)
+// sizes the per-env shared arrays.  The whole AbstractEnv.step — every substep of
 // Road.act/Road.step, then observe/reward/termination — runs in ONE kernel, so the SoA state
 // makes one HBM round trip per env-step (128-bit loads/stores per vehicle).
 //
@@ -21,7 +22,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <algorithm>
 #include <atomic>
+#include <cstddef>
 #include <mutex>
 
 #include <cuda_runtime.h>
@@ -101,6 +104,38 @@ __device__ __forceinline__ void env_sync_phase() {
 template <int NW>
 __device__ __forceinline__ bool test_bit(const uint32_t (&m)[NW], int i) {
     return (m[i >> 5] >> (i & 31)) & 1u;
+}
+
+// Hardware lane, read afresh at each use: a lane index held in a register across the substep loop costs a spill.
+__device__ __forceinline__ int lane_id() {
+    int l;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+    return l;
+}
+
+// Dense env segments (DENSE step kernels) in a warp.  A warp ballot is indexed by hardware lane, an env's mask words
+// by vehicle (bit i & 31 of word i >> 5), and a dense segment starts anywhere in a warp, so a warp holds parts of up
+// to three envs.  The first lane of each env's part (vehicle i, lane 0 or i == 0) ORs the part's bits, vehicles
+// [i, i + n), into the at most two words they straddle, which must be zero before.  Threads that own no vehicle
+// (i >= V) are never a first lane.
+__device__ __forceinline__ void segment_or(uint32_t* words, uint32_t ballot, int i, int V) {
+    const int lane = lane_id();
+    if (i >= V || (i != 0 && lane != 0)) return;
+    const int n = min(V - i, 32 - lane);
+    const uint32_t m = (ballot >> lane) & (0xffffffffu >> (32 - n));
+    if (!m) return;
+    const int sh = i & 31;
+    atomicOr(&words[i >> 5], m << sh);
+    const uint32_t hi = __funnelshift_l(m, 0u, sh);  // m >> (32 - sh), 0 for sh == 0
+    if (hi) atomicOr(&words[(i >> 5) + 1], hi);
+}
+// The env segments of the calling warp as a ballot of their first lanes, and the index of the caller's segment among
+// them (threads past the last env count as part of the last segment).  Warp-wide.
+__device__ __forceinline__ uint32_t segment_leads(int i, bool active, int& mine) {
+    const int lane = lane_id();
+    const uint32_t lead = __ballot_sync(0xffffffffu, active && (i == 0 || lane == 0));
+    mine = __popc(lead & (0xffffffffu >> (31 - lane))) - 1;
+    return lead;
 }
 
 // ------------------------------------------------------------------ neighbour search
@@ -330,7 +365,8 @@ __device__ __noinline__ void kinematics_row_features(const HwyHighwayParams& P, 
     }
 }
 
-template <int TPE>
+// DENSE (dense step kernels): threads i >= V own no vehicle and store nothing; the V threads pad the missing rows.
+template <int TPE, bool DENSE = false>
 __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, const Frame<TPE>& F,
                                                    double* key_scratch, int i, double heading,
                                                    float* __restrict__ obs_env,
@@ -346,7 +382,7 @@ __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, co
         ok = ok && (P.obs_see_behind || -2 * kVehLength < d);
         if (ok) key = fabs(d);
     }
-    key_scratch[i] = key;
+    if (!DENSE || i < V) key_scratch[i] = key;
     env_sync<TPE>();
     // stable rank among the valid candidates (python sorted() on |lane_distance_to|)
     int rank = 0, n_valid = 0;
@@ -356,7 +392,8 @@ __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, co
         rank += (ku < key) || (ku == key && u < i);
     }
     // obs_env == nullptr: an env of the block that is not observed (masked out, a surplus slot of the last block, not
-    // re-spawned).  It still runs to here so that every thread of the block meets the same barrier instruction.
+    // re-spawned), or in a dense kernel a thread that owns no vehicle.  It still runs to here so that every thread of
+    // the block meets the same barrier instruction.
     if (!obs_env) return;
     const double xr = 5.0 * kMaxSpeed, yr = 4.0 * P.lanes_count, vr = 2 * kMaxSpeed;
     int row = -1;
@@ -413,7 +450,15 @@ __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, co
         }
     }
     int filled = 1 + (n_valid < K - 1 ? n_valid : K - 1);  // zero padding of missing rows
-    if (i < K && i >= filled) {
+    if constexpr (DENSE) {
+        for (int pad = i; i < V && pad < K; pad += V) {  // (K may exceed V)
+            if (pad < filled) continue;
+            for (int col = 0; col < NF; ++col) {
+                obs_env[NF * pad + col] = 0.0f;
+                if (obs_env2) obs_env2[NF * pad + col] = 0.0f;
+            }
+        }
+    } else if (i < K && i >= filled) {
         for (int col = 0; col < NF; ++col) {
             obs_env[NF * i + col] = 0.0f;
             if (obs_env2) obs_env2[NF * i + col] = 0.0f;
@@ -453,8 +498,8 @@ __device__ __forceinline__ void store_vehicle(const HwyHighwayState& S, size_t s
 }
 
 // Stage one vehicle into frame F (plain stores) and clear the words of F that build_frame fills
-// with atomics.  Callers put a barrier between publish() and build_frame().
-template <int TPE, bool LINEAR = false>
+// with atomics (DENSE: the caller does, clear_masks).  Callers put a barrier between publish() and build_frame().
+template <int TPE, bool LINEAR = false, bool DENSE = false>
 __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F, int i, bool active,
                                         const VehicleRegs& r) {
     constexpr int NW = TPE / 32;
@@ -474,11 +519,22 @@ __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F
         F.lane[i] = (unsigned char)meta_lane(r.meta);
         F.tgt[i] = (unsigned char)meta_target(r.meta);
     }
-    if (i < HWY_MAX_LANES * NW) (&F.smask[0][0])[i] = 0;
+    if (!DENSE && i < HWY_MAX_LANES * NW) (&F.smask[0][0])[i] = 0;
     if (i == 0) {
         F.slow = 0;
         F.vmax_bits = 0u;
     }
+}
+
+// Dense step kernels: zero the words build_frame ORs into (smask, tm, lane_is, fired: adjacent in Frame), spread over
+// the env's V threads.
+template <int TPE>
+__device__ __forceinline__ void clear_masks(Frame<TPE>& F, int i, int V) {
+    constexpr int kWords = (3 * HWY_MAX_LANES + 1) * (TPE / 32);
+    static_assert(offsetof(Frame<TPE>, fired) + sizeof(F.fired) - offsetof(Frame<TPE>, smask) == 4 * kWords,
+                  "mask words of Frame are not adjacent");
+#pragma unroll 1  // (unrolled, it costs the step kernel 70 B of spills)
+    for (int k = i; k < kWords; k += V) (&F.smask[0][0])[k] = 0;
 }
 
 // Collision test of the pair a < b on the staged positions (vehicle/objects.py:92-138):
@@ -581,26 +637,62 @@ __device__ __noinline__ int rank_count(const Frame<TPE>& F, int V, int i, bool a
 // a strictly increasing chain of float keys — hence of the doubles — and every vehicle's rank is its old one, +-1 for
 // the swapped ones.  Like the chain check this runs redundantly in every warp of the env on shared data (ballots, no
 // barrier, no shared-memory writes), ~70 instructions instead of the ~400 of rank_count.  Returns the rank, or -1 when
-// the pattern is anything else (rank_count decides).  Boundary k = 32 w + b + 1 is bit b of word w.
-template <int TPE>
+// the pattern is anything else (rank_count decides).  Boundary k = 32 w + b + 1 is bit b of word w.  DENSE: the warp
+// evaluates each env segment it holds in turn, lane b taking boundaries 32 w + b + 1 of that env.
+template <int TPE, bool DENSE>
 __device__ __noinline__ int rank_repair(const Frame<TPE>& F, const Frame<TPE>& prev, int V, int i, bool active) {
     constexpr int NW = TPE / 32;
-    const int wl = i & 31;
     uint32_t inv[NW];
     uint32_t bad = 0;
+    if constexpr (!DENSE) {
+        const int wl = i & 31;
 #pragma unroll
-    for (int w = 0; w < NW; ++w) {
-        const int k = w * 32 + wl + 1;
-        const bool in = k < V;
-        const float a = in ? F.lsf[prev.perm[k - 1]] : 0.0f, c = in ? F.lsf[prev.perm[k]] : 1.0f;
-        bool wrong = in && !(a < c) && !(a > c);  // equal (or NaN) keys: not this path
-        if (in && a > c) {
-            // the swapped pair against its outer neighbours (positions k-2 and k+1 are unmoved, see the spacing rule)
-            if (k >= 2 && !(F.lsf[prev.perm[k - 2]] < c)) wrong = true;
-            if (k + 1 < V && !(a < F.lsf[prev.perm[k + 1]])) wrong = true;
+        for (int w = 0; w < NW; ++w) {
+            const int k = w * 32 + wl + 1;
+            const bool in = k < V;
+            const float a = in ? F.lsf[prev.perm[k - 1]] : 0.0f, c = in ? F.lsf[prev.perm[k]] : 1.0f;
+            bool wrong = in && !(a < c) && !(a > c);  // equal (or NaN) keys: not this path
+            if (in && a > c) {
+                // the swapped pair against its outer neighbours (positions k-2 and k+1 are unmoved, see the spacing
+                // rule)
+                if (k >= 2 && !(F.lsf[prev.perm[k - 2]] < c)) wrong = true;
+                if (k + 1 < V && !(a < F.lsf[prev.perm[k + 1]])) wrong = true;
+            }
+            inv[w] = __ballot_sync(0xffffffffu, in && a > c);
+            bad |= __ballot_sync(0xffffffffu, wrong);
         }
-        inv[w] = __ballot_sync(0xffffffffu, in && a > c);
-        bad |= __ballot_sync(0xffffffffu, wrong);
+    } else {
+        const int lane = lane_id();
+        int mine;
+        int s = 0;
+        for (uint32_t lead = segment_leads(i, active, mine); lead; lead &= lead - 1, ++s) {
+            // env of segment s: the envs of a block are consecutive EnvShared records
+            const ptrdiff_t d = (ptrdiff_t)(s - mine) * (ptrdiff_t)sizeof(EnvShared<TPE>);
+            const Frame<TPE>& Fs = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(&F) + d);
+            const Frame<TPE>& Ps = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(&prev) + d);
+            uint32_t s_inv[NW];
+            uint32_t s_bad = 0;
+#pragma unroll
+            for (int w = 0; w < NW; ++w) {
+                const int k = w * 32 + lane + 1;
+                const bool in = k < V;
+                const float a = in ? Fs.lsf[Ps.perm[k - 1]] : 0.0f, c = in ? Fs.lsf[Ps.perm[k]] : 1.0f;
+                bool wrong = in && !(a < c) && !(a > c);  // equal (or NaN) keys: not this path
+                if (in && a > c) {
+                    // the swapped pair against its outer neighbours (positions k-2 and k+1 are unmoved, see the spacing
+                    // rule)
+                    if (k >= 2 && !(Fs.lsf[Ps.perm[k - 2]] < c)) wrong = true;
+                    if (k + 1 < V && !(a < Fs.lsf[Ps.perm[k + 1]])) wrong = true;
+                }
+                s_inv[w] = __ballot_sync(0xffffffffu, in && a > c);
+                s_bad |= __ballot_sync(0xffffffffu, wrong);
+            }
+            if (s == mine) {
+#pragma unroll
+                for (int w = 0; w < NW; ++w) inv[w] = s_inv[w];
+                bad = s_bad;
+            }
+        }
     }
     // spacing: no other inverted boundary within two boundaries of an inverted one (also across the word seam)
 #pragma unroll
@@ -628,38 +720,67 @@ __device__ __noinline__ int rank_repair(const Frame<TPE>& F, const Frame<TPE>& p
 // After a barrier that follows publish(): ranks, rank-ordered membership masks, lane / target
 // masks (warp ballots) and the first pass of the collision sweep of Road.step
 // (road/road.py:477-481).  All threads of the env call this convergently.
-template <int TPE>
+template <int TPE, bool DENSE>
 __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared<TPE>& sm, Frame<TPE>& F,
                                             int i, bool active, bool aligned, const VehicleRegs& r,
                                             double dt, bool do_sweep, bool pruned, const Frame<TPE>* prev) {
     const int V = P.n_vehicles;
-    const int wie = i >> 5;  // warp within the env
+    const int wie = i >> 5;  // warp within the env (TPE-thread segments)
     const int lane = meta_lane(r.meta), tgt = meta_target(r.meta);
     // -- rank along the road (s, slot) and tie detection.  Float keys first: rounding to float
     // is monotone, so fu < fi implies su < si; only equal float keys need the doubles.
     int rank = 0;
     // The order along the road rarely changes within one substep: with the previous frame of the same launch at hand
-    // (`prev`, uniform), every warp of the env checks the whole chain key[perm[k-1]] < key[perm[k]] under the previous
-    // permutation (V - 1 float comparisons spread over its 32 lanes, no communication between the warps: each reaches
-    // the same verdict).  A strictly increasing chain of float keys is a strictly increasing chain of the doubles they
-    // were rounded from, so the ranks are the previous ones and there is neither a tie nor an ambiguity — the O(V)
-    // scan per thread (14 % of the kernel's instructions at V = 51) runs only when some pair swapped or drew level.
+    // (`prev`, uniform), every warp checks the whole chain key[perm[k-1]] < key[perm[k]] under the previous permutation
+    // of each env segment it holds, one with TPE-thread segments (V - 1 float comparisons spread over its 32 lanes, no
+    // communication between the warps: each warp of an env reaches the same verdict).  A strictly increasing chain of
+    // float keys is a strictly increasing chain of the doubles they were rounded from, so the ranks are the previous
+    // ones and there is neither a tie nor an ambiguity — the O(V) scan per thread (14 % of the kernel's instructions
+    // at V = 51) runs only when some pair swapped or drew level.
     bool reuse = false;
-    if (prev) {
+    if (prev && !DENSE) {
         bool ok = true;
 #pragma unroll 1
         for (int k = (i & 31) + 1; k < V; k += 32) ok = ok && (F.lsf[prev->perm[k - 1]] < F.lsf[prev->perm[k]]);
         reuse = __all_sync(0xffffffffu, ok);
+    } else if (prev) {
+        int mine, s = 0;
+#pragma unroll 1
+        for (uint32_t lead = segment_leads(i, active, mine); lead; lead &= lead - 1, ++s) {
+            // env of segment s: the envs of a block are consecutive EnvShared records
+            const ptrdiff_t d = (ptrdiff_t)(s - mine) * (ptrdiff_t)sizeof(EnvShared<TPE>);
+            const Frame<TPE>& Fs = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(&F) + d);
+            const Frame<TPE>& Ps = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(prev) + d);
+            bool ok = true;
+#pragma unroll 1
+            for (int k = lane_id() + 1; k < V; k += 32)
+                ok = ok && (Fs.lsf[Ps.perm[k - 1]] < Fs.lsf[Ps.perm[k]]);
+            ok = __all_sync(0xffffffffu, ok);
+            if (s == mine) reuse = ok;
+        }
     }
     bool tie = false;
-    if (reuse) {
-        rank = active ? prev->rank[i] : 0;
+    if constexpr (!DENSE) {
+        if (reuse) {
+            rank = active ? prev->rank[i] : 0;
+        } else {
+            // (the repair pays for itself only where the count is long, so only the 128-slot kernel uses it)
+            int rt = (TPE >= 128 && prev) ? rank_repair<TPE, DENSE>(F, *prev, V, i, active) : -1;
+            if (rt < 0) rt = rank_count(F, V, i, active);  // first frame of a launch, ties, or more than isolated swaps
+            rank = rt & 0xff;
+            tie = (rt >> 8) != 0;
+        }
     } else {
-        // (the repair pays for itself only where the count is long, so only the 128-slot kernel uses it)
-        int rt = (TPE >= 128 && prev) ? rank_repair(F, *prev, V, i, active) : -1;
-        if (rt < 0) rt = rank_count(F, V, i, active);  // first frame of a launch, ties, or more than isolated swaps
-        rank = rt & 0xff;
-        tie = (rt >> 8) != 0;
+        // the verdict differs between the segments of a warp, and the repair is warp-wide
+        int rt = -1;
+        if (TPE >= 128 && prev && __any_sync(0xffffffffu, !reuse)) rt = rank_repair<TPE, DENSE>(F, *prev, V, i, active);
+        if (reuse) {
+            rank = active ? prev->rank[i] : 0;
+        } else if (active) {
+            if (rt < 0) rt = rank_count(F, V, i, active);
+            rank = rt & 0xff;
+            tie = (rt >> 8) != 0;
+        }
     }
     if (active) {
         F.perm[rank] = (unsigned char)i;
@@ -678,7 +799,10 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     for (int l = 0; l < P.lanes_count; ++l) {
         uint32_t b_lane = __ballot_sync(0xffffffffu, active && lane == l);
         uint32_t b_tgt = __ballot_sync(0xffffffffu, active && tgt == l);
-        if ((i & 31) == 0) {
+        if constexpr (DENSE) {
+            segment_or(F.lane_is[l], b_lane, i, V);
+            segment_or(F.tm[l], b_tgt, i, V);
+        } else if ((i & 31) == 0) {
             F.lane_is[l][wie] = b_lane;
             F.tm[l][wie] = b_tgt;
         }
@@ -686,7 +810,10 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     // superset of the vehicles whose MOBIL decision may fire in the coming act (the crashed
     // flag may still be stale here; crashed vehicles never fire, so this only over-approximates)
     uint32_t b_fired = __ballot_sync(0xffffffffu, active && is_idm && lane == tgt && P.lane_change_delay < r.timer);
-    if ((i & 31) == 0) F.fired[wie] = b_fired;
+    if constexpr (DENSE)
+        segment_or(F.fired, b_fired, i, V);
+    else if ((i & 31) == 0)
+        F.fired[wie] = b_fired;
 
     // -- collision sweep, pass 1: every gated pair once.  A pair with exactly one
     // check_collisions side is taken by the other side's thread (so the controlled vehicle's
@@ -694,10 +821,19 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     if (do_sweep && pruned) {
         // many checking vehicles (highway-v0: all of them): the sweep runs after the next barrier over the
         // rank-neighbours only (sweep_pruned); here just the env's speed bound.  Non-negative floats order
-        // like their bit patterns.
-        unsigned vb = __float_as_uint(active ? fmaxf(__double2float_ru(r.speed), 0.0f) : 0.0f);
-        vb = __reduce_max_sync(0xffffffffu, vb);
-        if ((i & 31) == 0) atomicMax(&F.vmax_bits, vb);
+        // like their bit patterns.  DENSE: the reduction runs over the lanes of the caller's env segment in this warp.
+        if constexpr (DENSE) {
+            if (active) {
+                const int lane = lane_id(), lo = max(lane - i, 0), hi = min(lane - i + V, 32);
+                const unsigned vb = __reduce_max_sync((0xffffffffu >> (32 - (hi - lo))) << lo,
+                                                      __float_as_uint(fmaxf(__double2float_ru(r.speed), 0.0f)));
+                if (lane == lo) atomicMax(&F.vmax_bits, vb);
+            }
+        } else {
+            unsigned vb = __float_as_uint(active ? fmaxf(__double2float_ru(r.speed), 0.0f) : 0.0f);
+            vb = __reduce_max_sync(0xffffffffu, vb);
+            if ((i & 31) == 0) atomicMax(&F.vmax_bits, vb);
+        }
     } else if (active && do_sweep) {
         const bool cc_i = test_bit(sm.cc, i);
         auto do_pair = [&](int a, int b) {
@@ -1047,6 +1183,9 @@ constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full regis
 #endif
 
 // blockDim.x = TPE * (envs per block); dynamic shared memory = envs per block * sizeof(EnvShared).
+// DENSE (see launch_step): `dense_epb` envs per block, env `sub` on the V threads from sub * V, vehicle
+// i = threadIdx.x - sub * V; blockDim.x = dense_epb * V rounded up to whole warps, and the threads past dense_epb * V
+// own no vehicle: they meet every barrier and warp collective and do nothing else.
 // AL (host-checked, lanes_congruent): every lane is a copy of lane 0 shifted sideways — what
 // RoadNetwork.straight_road_network builds (road/road.py:291-321) — so the general-geometry branches (per-lane
 // projections in lane_distance / closest_lane, F.slow for unaligned lanes) are compiled out.  The per-substep loop
@@ -1057,28 +1196,28 @@ constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full regis
 // and highway_linear_step_kernel (LinearVehicle traffic, LINEAR = true, `T` its parameters; the block's LinearShared
 // staging follows its EnvShared array in dynamic shared memory).  Only `if constexpr (LINEAR)` branches differ, and
 // each kernel keeps the body in its own scope (an inlined device function changes the IDM kernel's code schedule).
-template <int TPE, bool AL>
+template <int TPE, bool AL, bool DENSE>
 __global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
 highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                     const int32_t* __restrict__ action_i, const float* __restrict__ action_f,
                     float* __restrict__ obs, double* __restrict__ reward,
                     uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
                     double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
-                    const int autoreset, float* __restrict__ final_obs) {
+                    const int autoreset, float* __restrict__ final_obs, const int dense_epb) {
     constexpr bool LINEAR = false;
     const HwyLinearTraffic* T = nullptr;
 #include "hwy_highway_step.cuh"
 }
 
 // LinearVehicle / AggressiveVehicle / DefensiveVehicle traffic (vehicle/behavior.py:350-583)
-template <int TPE, bool AL>
+template <int TPE, bool AL, bool DENSE>
 __global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
 highway_linear_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                            const __grid_constant__ HwyLinearTraffic T_, const int32_t* __restrict__ action_i,
                            const float* __restrict__ action_f, float* __restrict__ obs, double* __restrict__ reward,
                            uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
                            double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
-                           const int autoreset, float* __restrict__ final_obs) {
+                           const int autoreset, float* __restrict__ final_obs, const int dense_epb) {
     constexpr bool LINEAR = true;
     const HwyLinearTraffic* T = &T_;
 #include "hwy_highway_step.cuh"
@@ -1297,10 +1436,37 @@ Grid grid_for(int tpe, int n_envs) {
     return Grid{(n_envs + epb - 1) / epb, tpe * epb};
 }
 
-// Envs per block of the step kernel: as many as fit 512 threads (lock-step, see env_sync),
-// reduced when that leaves the last wave of blocks mostly empty.  HWYB200_EPB overrides.
-int step_envs_per_block(int tpe, int n_envs) {
-    int max_epb = (hwy::kMaxBlockThreads < HWY_STEP_BOUND_THREADS ? hwy::kMaxBlockThreads : HWY_STEP_BOUND_THREADS) / tpe;
+int step_block_thread_limit() {
+    return hwy::kMaxBlockThreads < HWY_STEP_BOUND_THREADS ? hwy::kMaxBlockThreads : HWY_STEP_BOUND_THREADS;
+}
+int step_half_block_threads() { return step_block_thread_limit() / 2; }
+// Envs per block of the step kernel: as many V-thread envs as fit half the block-thread limit (two blocks per SM),
+// reduced when that leaves the last wave of blocks mostly empty.  HWYB200_EPB overrides, up to the whole limit.  Both
+// are also bounded by shared memory (env_bytes per env), which only binds below V = 17.
+struct StepDevice {
+    int n_sm, smem_sm, smem_block;  // SMs, shared memory per SM, opt-in shared memory per block
+};
+// read once per device
+const StepDevice& step_device(int dev) {
+    static StepDevice info[64];
+    static std::atomic<bool> ready[64];
+    static std::mutex mu;
+    if (!ready[dev].load(std::memory_order_acquire)) {
+        std::lock_guard<std::mutex> lock(mu);
+        if (!ready[dev].load(std::memory_order_relaxed)) {
+            StepDevice d{132, 228 * 1024, 227 * 1024};
+            cudaDeviceGetAttribute(&d.n_sm, cudaDevAttrMultiProcessorCount, dev);
+            cudaDeviceGetAttribute(&d.smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+            cudaDeviceGetAttribute(&d.smem_block, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+            info[dev] = d;
+            ready[dev].store(true, std::memory_order_release);
+        }
+    }
+    return info[dev];
+}
+int step_envs_per_block(int n_vehicles, size_t env_bytes, int n_envs, const StepDevice& d) {
+    const int limit = step_block_thread_limit();
+    int max_epb = std::min<long>(limit / n_vehicles, d.smem_block / (long)env_bytes);
     if (max_epb < 1) max_epb = 1;
     if (const char* e = getenv("HWYB200_EPB")) {
         int v = atoi(e);
@@ -1308,11 +1474,9 @@ int step_envs_per_block(int tpe, int n_envs) {
     }
     // Two resident blocks per SM (rather than one block of max_epb envs or many 1-env blocks): the blocks cover each other's
     // barrier stalls.  Small batches shrink the block so every SM still gets work.
-    int n_sm = 132;
-    int dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    int epb = max_epb >= 2 ? max_epb / 2 : 1;
-    while (epb > 1 && (long)n_envs < (long)epb * 2 * n_sm) --epb;
+    int epb = std::min<long>(step_half_block_threads() / n_vehicles, (d.smem_sm / 2 - 1024) / (long)env_bytes);
+    if (epb < 1) epb = 1;
+    while (epb > 1 && (long)n_envs < (long)epb * 2 * d.n_sm) --epb;
     return epb;
 }
 
@@ -1360,35 +1524,55 @@ bool lanes_congruent_host(const HwyHighwayParams* p) {
     return ok;
 }
 
+template <int TPE, bool AL, bool DENSE>
+int launch_step_kernel(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                       const int32_t* action_i, const float* action_f, float* obs, double* reward,
+                       uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
+                       int autoreset, float* final_obs, int epb, size_t env_bytes, int dev, cudaStream_t st) {
+    const int blocks = (s->n_envs + epb - 1) / epb;
+    const size_t smem = (size_t)epb * env_bytes;
+    // the attribute is per device (and per template instance): cache it by device ordinal
+    static std::atomic<size_t> configured[2][64];
+    if (smem > configured[t != nullptr][dev].load(std::memory_order_relaxed)) {
+        cudaError_t err = t ? cudaFuncSetAttribute(hwy::highway_linear_step_kernel<TPE, AL, DENSE>,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                            : cudaFuncSetAttribute(hwy::highway_step_kernel<TPE, AL, DENSE>,
+                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
+        configured[t != nullptr][dev].store(smem, std::memory_order_relaxed);
+    }
+    const int threads = DENSE ? (epb * p->n_vehicles + 31) & ~31 : epb * TPE;
+    if (t)
+        hwy::highway_linear_step_kernel<TPE, AL, DENSE><<<blocks, threads, smem, st>>>(
+            *p, *s, *t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+            autoreset, final_obs, epb);
+    else
+        hwy::highway_step_kernel<TPE, AL, DENSE><<<blocks, threads, smem, st>>>(
+            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
+            autoreset, final_obs, epb);
+    return 0;
+}
+
 // t == nullptr: IDMVehicle traffic (highway_step_kernel); else LinearVehicle traffic (highway_linear_step_kernel)
 template <int TPE, bool AL>
 int launch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
                 const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
                 uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset,
-                float* final_obs, int blocks, int epb, cudaStream_t st) {
+                float* final_obs, cudaStream_t st) {
     if (autoreset > 0 && ensure_pcg_jump(st)) return 1;
-    size_t smem = (size_t)epb * (sizeof(hwy::EnvShared<TPE>) + (t ? sizeof(hwy::LinearShared<TPE>) : 0));
-    // the attribute is per device (and per template instance): cache it by device ordinal
-    static std::atomic<size_t> configured[2][64];
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
-    if (smem > configured[t != nullptr][dev].load(std::memory_order_relaxed)) {
-        cudaError_t err = t ? cudaFuncSetAttribute(hwy::highway_linear_step_kernel<TPE, AL>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                            : cudaFuncSetAttribute(hwy::highway_step_kernel<TPE, AL>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-        configured[t != nullptr][dev].store(smem, std::memory_order_relaxed);
-    }
-    if (t)
-        hwy::highway_linear_step_kernel<TPE, AL><<<blocks, TPE * epb, smem, st>>>(
-            *p, *s, *t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-            autoreset, final_obs);
-    else
-        hwy::highway_step_kernel<TPE, AL><<<blocks, TPE * epb, smem, st>>>(
-            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-            autoreset, final_obs);
-    return 0;
+    const size_t env_bytes = sizeof(hwy::EnvShared<TPE>) + (t ? sizeof(hwy::LinearShared<TPE>) : 0);
+    const int epb = step_envs_per_block(p->n_vehicles, env_bytes, s->n_envs, step_device(dev));
+    // Dense segments (V threads per env, the DENSE kernels) only where they put more envs into a block than TPE-thread
+    // segments; otherwise the TPE-thread kernel runs, which carries none of the segment bookkeeping.
+    const bool dense = epb * TPE > step_half_block_threads();
+    if (dense)
+        return launch_step_kernel<TPE, AL, true>(p, s, t, action_i, action_f, obs, reward, terminated, truncated,
+                                                 info_speed, info_crashed, autoreset, final_obs, epb, env_bytes, dev,
+                                                 st);
+    return launch_step_kernel<TPE, AL, false>(p, s, t, action_i, action_f, obs, reward, terminated, truncated,
+                                              info_speed, info_crashed, autoreset, final_obs, epb, env_bytes, dev, st);
 }
 
 int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask_a,
@@ -1585,14 +1769,12 @@ int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const Hwy
                   uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
                   cudaStream_t st) {
     int tpe = tpe_for(p->n_vehicles);
-    int epb = step_envs_per_block(tpe, s->n_envs);
-    int blocks = (s->n_envs + epb - 1) / epb;
     // HWYB200_GENERAL_LANES=1 (tests): run the general-geometry instantiation on a congruent lane table too
     const char* force_general = getenv("HWYB200_GENERAL_LANES");
     const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
 #define HWY_LAUNCH_STEP(T, A)                                                                              \
     launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
-                      autoreset, final_obs, blocks, epb, st)
+                      autoreset, final_obs, st)
     int rc;
     if (tpe == 32)
         rc = al ? HWY_LAUNCH_STEP(32, true) : HWY_LAUNCH_STEP(32, false);

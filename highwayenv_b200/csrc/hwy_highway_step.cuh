@@ -4,23 +4,32 @@
     constexpr int NW = TPE / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     EnvShared<TPE>* smem = reinterpret_cast<EnvShared<TPE>*>(smem_raw);
-    const int EPB = blockDim.x / TPE;
-    const int sub = threadIdx.x / TPE;
-    const int i = threadIdx.x % TPE;
+    const int V = P.n_vehicles;
+    // DENSE: env `sub` of the block owns the V threads from sub * V; the threads past EPB * V own no vehicle (i = V,
+    // active = false): they keep the last env's shared-memory address but neither load nor store.  Otherwise env
+    // `sub` owns the TPE threads from sub * TPE.
+    const int EPB = DENSE ? dense_epb : blockDim.x / TPE;
+    const int seg = threadIdx.x / (DENSE ? V : TPE);
+    const int sub = DENSE && seg >= EPB ? EPB - 1 : seg;
+    const int i = DENSE ? (seg < EPB ? threadIdx.x - seg * V : V) : threadIdx.x % TPE;
+    const bool active = i < V;
     const int env = blockIdx.x * EPB + sub;
-    const bool env_ok = env < S.n_envs;  // surplus envs of the last block mirror the last env
-    const int e = env_ok ? env : S.n_envs - 1;
+    const bool env_ok = (!DENSE || active) && env < S.n_envs;  // surplus envs of the last block mirror the last env
+    const int e = env < S.n_envs ? env : S.n_envs - 1;
     EnvShared<TPE>& sm = smem[sub];
     LinearShared<TPE>* lsm = nullptr;
     if constexpr (LINEAR) lsm = reinterpret_cast<LinearShared<TPE>*>(smem + EPB) + sub;
-    const int V = P.n_vehicles;
-    const bool active = i < V;
     const size_t slot = (size_t)e * S.vp + (active ? i : 0);
     const bool aligned = AL || lanes_aligned(P);
     const bool congruent = AL || lanes_congruent(P);
 
     VehicleRegs r;
-    load_vehicle(S, slot, r);
+    if constexpr (DENSE) {
+        r = {};
+        if (active) load_vehicle(S, slot, r);
+    } else {
+        load_vehicle(S, slot, r);
+    }
     const int kind = meta_kind(r.meta);
     int speed_index = (i == 0) ? S.speed_index[e] : 0;
     double act_steer = 0.0, act_accel = 0.0;
@@ -34,13 +43,21 @@
     {
         uint32_t b_cc = __ballot_sync(0xffffffffu, active && (r.meta & HWY_META_CHECK_COLLISIONS));
         uint32_t b_ctrl = __ballot_sync(0xffffffffu, active && kind != HWY_KIND_VEHICLE);
-        if ((i & 31) == 0) {
-            sm.cc[i >> 5] = b_cc;
-            sm.ctrl[i >> 5] = b_ctrl;
-            sm.mid[i >> 5] = 0;
+        if constexpr (DENSE) {
+            if (i < NW) sm.cc[i] = sm.ctrl[i] = sm.mid[i] = 0;
+            if (active) {
+                sm.last_will[i] = -1;
+                sm.crash_hit[i] = 0;
+            }
+        } else {
+            if ((i & 31) == 0) {
+                sm.cc[i >> 5] = b_cc;
+                sm.ctrl[i >> 5] = b_ctrl;
+                sm.mid[i >> 5] = 0;
+            }
+            sm.last_will[i] = -1;
+            sm.crash_hit[i] = 0;
         }
-        sm.last_will[i] = -1;
-        sm.crash_hit[i] = 0;
         if (i < NW) sm.ok_left[i] = sm.ok_right[i] = 0;
         if (i == 0) sm.n_items = 0;
         if (active) sm.delta[i] = r.delta;
@@ -50,6 +67,11 @@
                 for (int k = 0; k < 3; ++k) lsm->acc[k][i] = lp[k];
                 for (int k = 0; k < 2; ++k) lsm->steer[k][i] = lp[3 + k];
             }
+        }
+        if constexpr (DENSE) {
+            __syncthreads();  // (once per launch) the zeroed words before the env segments OR their bits in
+            segment_or(sm.cc, b_cc, i, V);
+            segment_or(sm.ctrl, b_ctrl, i, V);
         }
     }
     const IdmK K = make_idm(P);
@@ -65,7 +87,8 @@
     for (int frame = 0;; ++frame) {
         p ^= 1;
         Frame<TPE>& F = sm.f[p];
-        publish<TPE, LINEAR>(P, F, i, active, r);
+        publish<TPE, LINEAR, DENSE>(P, F, i, active, r);
+        if (DENSE && active) clear_masks(F, i, V);
         PHASE_MARK(1);  // publish
         env_sync<TPE>();
         PHASE_MARK(2);  // barrier after publish
@@ -73,7 +96,8 @@
         if (i == 0) sm.n_items = 0;
         // frame 0: masks only — the sweep of the stored state ran at the end of the substep that
         // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).
-        build_frame(P, sm, F, i, active, aligned, r, dt, frame > 0, pruned, frame > 0 ? &sm.f[p ^ 1] : nullptr);
+        build_frame<TPE, DENSE>(P, sm, F, i, active, aligned, r, dt, frame > 0, pruned,
+                                frame > 0 ? &sm.f[p ^ 1] : nullptr);
         PHASE_MARK(3);  // ranks, masks, sweep pass 1
         if (pruned && frame > 0) {  // uniform over the grid
             env_sync_phase<TPE, 3>();
@@ -207,7 +231,7 @@
         // branch) for the queued (vehicle, candidate) items, one item per thread.
         if constexpr (LINEAR) {
             // the same with LinearVehicle.acceleration (behavior.py:417-465) and the item owner's parameters
-            for (int t = i; t < sm.n_items; t += TPE) {
+            for (int t = i; (!DENSE || active) && t < sm.n_items; t += DENSE ? V : TPE) {
                 const int it = sm.items[t];
                 const int v = it & 0xff, cand = (it >> 8) & 0x7f, right = it >> 15;
                 const double a0 = lsm->acc[0][v], a1 = lsm->acc[1][v], a2 = lsm->acc[2][v];
@@ -233,7 +257,7 @@
                 atomicOr(right ? &sm.ok_right[v >> 5] : &sm.ok_left[v >> 5], 1u << (v & 31));
             }
         } else
-        for (int t = i; t < sm.n_items; t += TPE) {
+        for (int t = i; (!DENSE || active) && t < sm.n_items; t += DENSE ? V : TPE) {
             const int it = sm.items[t];
             const int v = it & 0xff, cand = (it >> 8) & 0x7f, right = it >> 15;
             const double delta_v = sm.delta[v];
@@ -395,7 +419,7 @@
     const Frame<TPE>& F = sm.f[p];
     const size_t obs_off = (size_t)e * P.obs_vehicles_count * obs_columns(P);
     float* obs_env = obs + obs_off;
-    kinematics_observe(P, F, sm.key, i, r.heading, env_ok ? obs_env : nullptr,
+    kinematics_observe<TPE, DENSE>(P, F, sm.key, i, r.heading, env_ok ? obs_env : nullptr,
                        (autoreset && final_obs) ? final_obs + obs_off : nullptr);
     if (i == 0) {
         sm.done = 0;
@@ -447,13 +471,13 @@
         const bool simple_geometry = aligned && P.lanes[0].start_x == 0.0 && P.lanes[0].dir_x == 1.0;
         spawn_fused<TPE, LINEAR>(P, S, sm, e, i, active, do_reset, simple_geometry, r, speed_index, T);
         Frame<TPE>& G = sm.f[p ^ 1];
-        if (do_reset) publish(P, G, i, active, r);
+        if (do_reset) publish<TPE, false, DENSE>(P, G, i, active, r);
         // barrier + "does any env of this block re-spawn?": the second observation runs under a block-uniform
         // condition, so that all threads of the block meet the same barrier instructions (a per-env condition around
         // __syncthreads() is what compute-sanitizer's synccheck rejects, even though the arrival counts match)
         const bool any_reset = __syncthreads_or(do_reset) != 0;
         if (any_reset) {
-            kinematics_observe(P, G, sm.key, i, r.heading, do_reset ? obs_env : nullptr);
+            kinematics_observe<TPE, DENSE>(P, G, sm.key, i, r.heading, do_reset ? obs_env : nullptr);
             if (do_reset && i == 0) {
                 S.time[e] = 0.0;
                 S.speed_index[e] = speed_index;
