@@ -252,6 +252,20 @@ class HwyValueIterationParams(C.Structure):
                 ("gamma", C.c_double), ("state", C.c_void_p), ("action", C.c_void_p)]
 
 
+HWY_COPY_MAX_BUFS = 32
+
+
+class HwyRowCopy(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_bytes", C.c_int64)]
+
+
+class HwyOpdTree(C.Structure):
+    _fields_ = ([("n_roots", C.c_int32), ("max_nodes", C.c_int32), ("expansions", C.c_int32), ("n_actions", C.c_int32)]
+                + [(n, C.c_void_p) for n in ("discount", "bound", "exists", "expanded", "terminal", "parent", "action",
+                                             "depth", "branch", "reward", "value", "upper", "selected", "leaf_row",
+                                             "recommended")])
+
+
 class HwyLidarParams(C.Structure):
     _fields_ = [("cells", C.c_int32), ("normalize", C.c_int32), ("maximum_range", C.c_double)]
 
@@ -265,7 +279,8 @@ EXPORTS = (
     "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
     "hwy_value_iteration", "hwy_highway_linear_reset", "hwy_highway_linear_step", "hwy_highway_linear_autoreset",
-    "hwy_highway_linear_substeps",
+    "hwy_highway_linear_substeps", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
+    "hwy_opd_recommend",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -370,6 +385,17 @@ def load():
     lib.hwy_finite_mdp.argtypes = [NG, OV, C.POINTER(HwyFiniteMdpParams)] + [C.c_void_p] * 8
     lib.hwy_value_iteration.restype = C.c_int
     lib.hwy_value_iteration.argtypes = [C.POINTER(HwyValueIterationParams)] + [C.c_void_p] * 7
+    lib.hwy_copy_env_rows.restype = C.c_int
+    lib.hwy_copy_env_rows.argtypes = [C.POINTER(HwyRowCopy), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    lib.hwy_available_actions.restype = C.c_int
+    lib.hwy_available_actions.argtypes = [NG, OV, C.c_int, C.c_void_p, C.c_void_p]
+    OT = C.POINTER(HwyOpdTree)
+    lib.hwy_opd_select.restype = C.c_int
+    lib.hwy_opd_select.argtypes = [OT, C.c_int, C.c_void_p]
+    lib.hwy_opd_record.restype = C.c_int
+    lib.hwy_opd_record.argtypes = [OT, C.c_int] + [C.c_void_p] * 5
+    lib.hwy_opd_recommend.restype = C.c_int
+    lib.hwy_opd_recommend.argtypes = [OT, C.c_void_p]
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

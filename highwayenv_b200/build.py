@@ -10,14 +10,14 @@ import subprocess
 import sys
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = [os.path.join(_HERE, "csrc", f) for f in ("hwy_highway.cu", "hwy_network.cu", "hwy_observe.cu", "hwy_plan.cu")]
+SRC = [os.path.join(_HERE, "csrc", f) for f in ("hwy_highway.cu", "hwy_network.cu", "hwy_observe.cu", "hwy_plan.cu", "hwy_copy.cu")]
 DEPS = SRC + [os.path.join(_HERE, "csrc", h) for h in ("hwy_math.cuh", "hwy_device.cuh", "hwy_lanes.cuh", "hwy_abi.h", "hwy_highway_step.cuh", "hwy_highway_reset.cuh")] + [
     os.path.join(os.path.dirname(_HERE), "include", "hwyb200.h")]
 OUT = os.path.join(_HERE, "csrc", "libhwyb200.so")
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
-    "-fmad=false", "-Xcompiler", "-fPIC", "-shared", "--threads", "4",  # the four sources compile concurrently
+    "-fmad=false", "-Xcompiler", "-fPIC", "-shared", "--threads", "5",  # the five sources compile concurrently
 ]
 
 

@@ -257,6 +257,106 @@ class BatchedVectorEnv:
             return self._obs.to(torch.uint8)
         return self._obs
 
+    # ------------------------------------------------------------------ cloning
+    # tensors with a leading num_envs axis that copy_envs leaves alone: per-step outputs (a later call overwrites them
+    # before it reads them), scratch and staging buffers
+    ROW_EXCLUDE = frozenset({
+        "_final_obs", "_fused_out", "_reward", "_terminated", "_truncated", "_info_speed", "_info_crashed",
+        "_reward_terms", "_action_buf", "_mask_keepalive", "_agents_reward", "_agents_terminated"})
+
+    def _env_rows(self) -> dict:
+        """Every per-env tensor a later call reads, as name -> a [num_envs, ...] view: the state copy_envs copies.
+        The streams are [5, num_envs] and appear transposed; the NextStep pending-reset flag appears once it exists."""
+        n = self.num_envs
+        rows = {"_pos": self._pos, "_hs": self._hs, "_tt": self._tt, "_imp": self._imp, "_delta": self._delta,
+                "_meta": self._meta, "_speed_index": self._speed_index.view(n, -1), "_time": self._time,
+                "_rng": self._rng.t(), "_obs": self._obs}
+        if self._autoreset_envs is not None:
+            rows["_autoreset_envs"] = self._autoreset_envs
+        return rows
+
+    def _row_layout(self) -> dict:
+        rows = self._env_rows()
+        rows.pop("_autoreset_envs", None)
+        return {k: (tuple(t.shape[1:]), t.dtype) for k, t in rows.items()}
+
+    def _row_copy_table(self, source) -> "C.Array":
+        """The HwyRowCopy entries that copy rows of `source` into rows of this env (one per contiguous row buffer)."""
+        dst_rows, src_rows = self._env_rows(), source._env_rows()
+        if "_autoreset_envs" in dst_rows and "_autoreset_envs" not in src_rows:  # no reset pending in the source
+            src_rows["_autoreset_envs"] = torch.zeros_like(dst_rows["_autoreset_envs"])
+            self._flag_keepalive = src_rows["_autoreset_envs"]
+        pairs = []
+        for name, d in dst_rows.items():
+            s = src_rows[name]
+            if d.dim() == 2 and not (d.is_contiguous() and s.is_contiguous()):  # [n, k] views of [k, n]: per column
+                pairs += [(s[:, j], d[:, j]) for j in range(d.shape[1])]
+            else:
+                pairs.append((s, d))
+        table = (N.HwyRowCopy * len(pairs))()
+        for e, (s, d) in zip(table, pairs):
+            assert s.is_contiguous() and d.is_contiguous() and s[0].numel() == d[0].numel()
+            e.src, e.dst, e.row_bytes = s.data_ptr(), d.data_ptr(), d[0].numel() * d.element_size()
+        return table
+
+    def _available_actions(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """DiscreteMetaAction.get_available_actions of every env on the device (hwy_available_actions): a bool mask
+        [N, 5] over (LANE_LEFT, IDLE, LANE_RIGHT, FASTER, SLOWER), written into `out` (uint8 [N, 5]) when given."""
+        if out is None:
+            out = torch.empty(self.num_envs, 5, dtype=torch.uint8, device=self.device)
+        view, graph = self._obs_view()
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_available_actions(graph, C.byref(view), int(self._params.n_target_speeds),
+                                                    out.data_ptr(), self._stream()))
+        return out.view(torch.bool)
+
+    def _copy_rows(self, table, dst: torch.Tensor, src: torch.Tensor) -> None:
+        """One hwy_copy_env_rows launch, without checks (dst, src: device int64 [n_pairs])."""
+        if dst.numel() == 0:
+            return
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_copy_env_rows(table, len(table), dst.data_ptr(), src.data_ptr(), dst.numel(),
+                                                self._stream()))
+
+    def _index_tensor(self, ids) -> torch.Tensor:
+        t = ids if isinstance(ids, torch.Tensor) else torch.from_numpy(np.asarray(ids, dtype=np.int64))
+        return t.to(device=self.device, dtype=torch.int64).reshape(-1).contiguous()
+
+    def copy_envs(self, dst_ids, src_ids, source=None) -> None:
+        """Copy the complete state of envs `src_ids` of `source` (default: this env) into envs `dst_ids` of this env.
+        Afterwards env dst_ids[k] behaves as `copy.deepcopy` of env src_ids[k] would: the same future under the same
+        actions, streams included.  One kernel launch; device int64 index tensors make it capturable in a CUDA graph.
+
+        Raises before any launch when `source` has another class or layout (vehicles, slots, observation shape, traffic
+        model, agents, device) or the index lists differ in length; outside stream capture also when an index is out
+        of range, `dst_ids` repeats an env, or (within one env) an env is both a source and a destination.  A
+        destination env never seeded is seeded first, as load_state_dict does."""
+        source = self if source is None else source
+        if type(source) is not type(self):
+            raise TypeError(f"copy_envs from a {type(source).__name__} into a {type(self).__name__}")
+        if not source._seeded:
+            raise RuntimeError("call reset() on the source before copy_envs()")
+        if source.device != self.device or source.V != self.V or source._row_layout() != self._row_layout() \
+                or source.config.get("other_vehicles_type") != self.config.get("other_vehicles_type"):
+            raise ValueError("copy_envs between envs of different layouts (vehicles, observation, traffic model, "
+                             "agents or device)")
+        dst, src = self._index_tensor(dst_ids), self._index_tensor(src_ids)
+        if dst.numel() != src.numel():
+            raise ValueError("dst_ids and src_ids must have the same length")
+        if not torch.cuda.is_current_stream_capturing() and dst.numel():  # reads the indices: one host round trip
+            d, s = dst.cpu().numpy(), src.cpu().numpy()
+            if d.min() < 0 or d.max() >= self.num_envs or s.min() < 0 or s.max() >= source.num_envs:
+                raise IndexError("env index out of range")
+            if np.unique(d).size != d.size:
+                raise ValueError("dst_ids repeats an env")
+            if source is self and np.intersect1d(d, s).size:
+                raise ValueError("an env is both a source and a destination")
+        if not self._seeded:
+            self._seed_streams(0)
+        if self.autoreset_mode == "NextStep" and self._autoreset_envs is None:
+            self._autoreset_envs = torch.zeros(self.num_envs, dtype=torch.uint8, device=self.device)
+        self._copy_rows(self._row_copy_table(source), dst, src)
+
     # ------------------------------------------------------------------ state import / export
     def state_dict(self) -> dict:
         """Per-field numpy arrays [N, V] (the reference's per-vehicle attributes), speed index, clock and streams."""
@@ -360,6 +460,14 @@ class BatchedNetworkEnv(BatchedVectorEnv):
         st.reward_terms = self._reward_terms.data_ptr()
         self._state = st
         return st
+
+    def _env_rows(self) -> dict:
+        rows = super()._env_rows()
+        rows.update({"_route": self._route, "_route_len": self._route_len})
+        for name in ("_count", "_road_steps", "_overflow"):  # the 32-slot kernels' population and rule clock
+            if getattr(self, name, None) is not None:
+                rows[name] = getattr(self, name)
+        return rows
 
     def _route_tables(self, destinations):
         """plan_route_to(lane, destination) (vehicle/controller.py:71-87) for every lane, on the device; returns the

@@ -309,6 +309,12 @@ class BatchedHighwayEnv(BatchedVectorEnv):
                 N.check(self._lib.hwy_highway_substeps(C.byref(self._params), C.byref(self._state), int(n_substeps),
                                                        af, self._stream()))
 
+    def _env_rows(self) -> dict:
+        rows = super()._env_rows()
+        if self._traffic is not None:
+            rows["_linear_params"] = self._linear_params
+        return rows
+
     # ------------------------------------------------------------------ state import / export
     def state_dict(self) -> dict:
         """The base fields; with LinearVehicle traffic also every vehicle's ``acceleration_parameters`` [N, V, 3] and

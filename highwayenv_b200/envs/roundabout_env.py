@@ -246,6 +246,14 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
                     self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
                     self._stream()))
 
+    def get_available_actions(self) -> torch.Tensor:
+        """DiscreteMetaAction.get_available_actions (envs/common/action.py:262-298, AbstractEnv.get_available_actions
+        abstract.py:357-358) for every env at once, on the device: a bool mask [N, 5] over (LANE_LEFT, IDLE,
+        LANE_RIGHT, FASTER, SLOWER).  A lane change is available when the side lane exists on the ego's road and
+        `is_reachable_from` the ego's position (road/lane.py:104-118, circular and sine lanes included); FASTER /
+        SLOWER unless the speed index sits at the end of `target_speeds`."""
+        return self._available_actions()
+
     # ------------------------------------------------------------------ host-exact reset
     def _reset_envs(self, env_ids: np.ndarray) -> None:
         sp = self.spawner.spawn([self._rngs[e] for e in env_ids])

@@ -11,10 +11,18 @@ rl-agents' `ValueIterationAgent`, and the policy that rebuilds and solves the MD
 `env.to_finite_mdp()` (csrc/hwy_observe.cu finite_mdp_kernel) builds, per env, the time-to-collision grid over every
 lane of the ego's road and the deterministic MDP on its (speed, lane, time) cells; `value_iteration()`
 (csrc/hwy_plan.cu) solves any batch of deterministic MDPs in that layout.
+
+`OpdPolicy` plans on the simulator itself instead of the TTC abstraction: optimistic deterministic planning over
+clones of every env (`env.copy_envs`, csrc/hwy_copy.cu), with its tree kernels in csrc/hwy_plan.cu.
+
+    policy = OpdPolicy(env, budget=50, gamma=0.7)
+    env.step(policy.act())
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -236,4 +244,117 @@ class TtcValueIterationPolicy:
         _launch_finite_mdp(env, p, m)
         _launch_value_iteration(m.transition, m.reward, m.terminal, m.n_states, self.gamma, self.iterations, self.q,
                                 self.iterations_done, m.state, self.actions)
+        return self.actions
+
+
+OPD_ENV_IDS = ("highway-v0", "highway-fast-v0", "roundabout-v0", "roundabout-v1", "merge-v0", "merge-v1", "exit-v0",
+               "exit-v1")
+
+
+def opd_discount_tables(gamma: float, expansions: int):
+    """(g, t) float64 [expansions + 2]: g[d] = gamma ** d and the optimistic bound t[d] = g[d] / (1 - gamma) of the
+    discounted rewards past depth d (rewards <= 1)."""
+    g = np.float64(gamma) ** np.arange(expansions + 2, dtype=np.float64)
+    return g, g / (np.float64(1.0) - np.float64(gamma))
+
+
+class OpdPolicy:
+    """Optimistic deterministic planning (Hren & Munos 2008; rl-agents' `DeterministicPlannerAgent`, which the
+    reference's quickstart runs on highway-fast-v0 with `budget: 50, gamma: 0.7`) on the simulator itself, for every
+    env of a batched env at once.  The statement it follows is tests/opd_spec.py.
+
+    Per root env, a tree of M = 1 + 5 E nodes (E = budget // 5 expansions) lives in a *store* env of N * M rows, one
+    per node; a *work* env of N * 5 rows steps a leaf's state once per action.  Expansion k:
+
+      1. hwy_opd_select picks, per root, the open leaf with the largest upper bound;
+      2. work.copy_envs: the leaf's store row into the root's 5 work rows;
+      3. the leaf's available actions (hwy_available_actions) and work.step(0..4);
+      4. store.copy_envs: the work rows into the child rows 1 + 5 k + a;
+      5. hwy_opd_record writes the children's records.
+
+    `act()` returns int64 actions [N] on the env's device: the root child whose subtree holds the largest value.
+    Buffers and the two envs are built at the first call (and again only if the env's size changes); later calls make
+    no host synchronisation and no allocation, so `act()` can be captured in a CUDA graph.  `tree` holds the last
+    decision's trees as [N, M] device tensors (exists, parent, action, depth, reward, value, upper, terminal,
+    expanded) and `selected` [N, E]."""
+
+    def __init__(self, env, budget: int = 50, gamma: float = 0.7):
+        from .envs.common.action import DiscreteMetaAction
+
+        if getattr(env, "multi_agent", False) or getattr(env, "n_agents", 1) > 1:
+            raise NotImplementedError("OPD of a multi-agent env")
+        if env.ENV_ID not in OPD_ENV_IDS:
+            raise NotImplementedError(f"OPD on {env.ENV_ID} (supported: {', '.join(OPD_ENV_IDS)})")
+        if not isinstance(getattr(env, "action_type", None), DiscreteMetaAction):
+            raise ValueError("OPD plans over the 5 DiscreteMetaAction actions of an MDPVehicle ego")
+        if not 0.0 <= float(gamma) < 1.0:
+            raise ValueError("gamma must be in [0, 1)")
+        if int(budget) != budget or budget < N_ACTIONS:
+            raise ValueError(f"budget must be an int >= {N_ACTIONS} (the number of actions)")
+        self.env, self.budget, self.gamma = env, int(budget), float(gamma)
+        self.expansions = self.budget // N_ACTIONS
+        self.max_nodes = 1 + N_ACTIONS * self.expansions
+        self._key = None
+        self.store = self.work = self.tree = self.selected = self.actions = None
+
+    def _allocate(self) -> None:
+        env, n, M, E, dev = self.env, self.env.num_envs, self.max_nodes, self.expansions, self.env.device
+        cls, cfg = type(env), copy.deepcopy(env.config)
+        self.store = cls(config=cfg, num_envs=n * M, device=dev, autoreset_mode="Disabled")
+        self.work = cls(config=copy.deepcopy(cfg), num_envs=n * N_ACTIONS, device=dev, autoreset_mode="Disabled")
+        # every row is written by copy_envs before anything reads it: no streams to seed
+        self.store._seeded = self.work._seeded = True
+        z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=dev)  # noqa: E731
+        g, t = opd_discount_tables(self.gamma, E)
+        self._g, self._t = torch.from_numpy(g).to(dev), torch.from_numpy(t).to(dev)
+        tr = {name: z(n, M, dtype=torch.uint8) for name in ("exists", "expanded", "terminal")}
+        tr.update({name: z(n, M, dtype=torch.int32) for name in ("parent", "action", "depth", "branch")})
+        tr.update({name: z(n, M, dtype=torch.float64) for name in ("reward", "value", "upper")})
+        self._buffers = tr
+        self.selected = z(n, E, dtype=torch.int32)
+        self.actions = z(n, dtype=torch.int64)
+        self._leaf_row = z(n * N_ACTIONS, dtype=torch.int64)
+        self._available = z(n * N_ACTIONS, N_ACTIONS, dtype=torch.uint8)
+        T = N.HwyOpdTree()
+        T.n_roots, T.max_nodes, T.expansions, T.n_actions = n, M, E, N_ACTIONS
+        T.discount, T.bound = self._g.data_ptr(), self._t.data_ptr()
+        for name, buf in tr.items():
+            setattr(T, name, buf.data_ptr())
+        T.selected, T.leaf_row, T.recommended = self.selected.data_ptr(), self._leaf_row.data_ptr(), self.actions.data_ptr()
+        self._T = T
+        self.tree = SimpleNamespace(**{k: (v.view(torch.bool) if v.dtype == torch.uint8 else v) for k, v in tr.items()},
+                                    selected=self.selected)
+        # row indices: root r -> store row r M; work row r 5 + a; child of expansion k -> store row r M + 1 + 5 k + a
+        roots = torch.arange(n, dtype=torch.int64, device=dev)
+        self._root_src, self._root_dst = roots, roots * M
+        self._work_rows = torch.arange(n * N_ACTIONS, dtype=torch.int64, device=dev)
+        a = torch.arange(N_ACTIONS, dtype=torch.int64, device=dev)
+        self._child_rows = [((roots * M)[:, None] + 1 + N_ACTIONS * k + a[None, :]).reshape(-1).contiguous()
+                            for k in range(E)]
+        self._work_actions = a.to(torch.int32).repeat(n)
+        self._leaf_table = self.work._row_copy_table(self.store)
+        self._child_table = self.store._row_copy_table(self.work)
+        self._key = (n, dev, env.V, str(env._row_layout()))
+
+    def act(self) -> torch.Tensor:
+        env = self.env
+        if not env._seeded:
+            raise RuntimeError("call reset() before act()")
+        if (env.num_envs, env.device, env.V, str(env._row_layout())) != self._key:
+            self._allocate()
+        store, work, lib, T = self.store, self.work, env._lib, C.byref(self._T)
+        # the root states into node 0, unchecked (the checks of copy_envs read the indices back); the env's buffers may
+        # have been re-allocated since the last call, so its table is built again
+        store._copy_rows(store._row_copy_table(env), self._root_dst, self._root_src)
+        stream = env._stream()
+        with torch.cuda.device(env.device):
+            for k in range(self.expansions):
+                N.check(lib.hwy_opd_select(T, k, stream))
+                work._copy_rows(self._leaf_table, self._work_rows, self._leaf_row)
+                work._available_actions(self._available)
+                work.step(self._work_actions)
+                store._copy_rows(self._child_table, self._child_rows[k], self._work_rows)
+                N.check(lib.hwy_opd_record(T, k, self._available.data_ptr(), work._reward.data_ptr(),
+                                           work._terminated.data_ptr(), work._truncated.data_ptr(), stream))
+            N.check(lib.hwy_opd_recommend(T, stream))
         return self.actions

@@ -620,6 +620,52 @@ typedef struct HwyLidarParams {
 int hwy_observe_lidar(const HwyObsView *view, const HwyLidarParams *p, const uint8_t *mask_a, const uint8_t *mask_b,
                       float *obs, void *stream);
 
+/* ====================================================================== env cloning and tree search
+ * Row copies between the per-env buffers of two env instances (or within one): for every pair k and every buffer b,
+ * bytes [dst[k] * row_bytes, (dst[k] + 1) * row_bytes) of bufs[b].dst take those of row src[k] of bufs[b].src.  One
+ * launch for all buffers; 16-byte vector copies where both rows and row_bytes are 16-byte aligned, 4-byte copies where
+ * they are 4-byte aligned, bytes otherwise.  dst [n_pairs], src [n_pairs] are DEVICE int64 row indices; the caller
+ * guarantees they are in range, that dst has no duplicates and that no row is both read and written. */
+#define HWY_COPY_MAX_BUFS 32
+typedef struct HwyRowCopy {
+    const void *src; /* DEVICE row 0 of the source buffer */
+    void *dst;       /* DEVICE row 0 of the destination buffer */
+    int64_t row_bytes;
+} HwyRowCopy;
+int hwy_copy_env_rows(const HwyRowCopy *bufs, int n_bufs, const int64_t *dst, const int64_t *src, int n_pairs,
+                      void *stream);
+
+/* DiscreteMetaAction.get_available_actions (envs/common/action.py:262-298) of the first controlled vehicle of every
+ * env on a lane table: mask [n_envs][5] u8 over (LANE_LEFT, IDLE, LANE_RIGHT, FASTER, SLOWER).  A side lane (id - 1,
+ * id + 1 on the ego's road, road/road.py:200-211) is available when it is_reachable_from the ego's position
+ * (road/lane.py:104-118); FASTER / SLOWER unless speed_index sits at the end of the n_target_speeds. */
+int hwy_available_actions(const HwyNetGraph *graph, const HwyObsView *view, int n_target_speeds, uint8_t *mask,
+                          void *stream);
+
+/* Optimistic deterministic planning (Hren & Munos 2008) over n_roots trees of max_nodes = 1 + 5 * expansions nodes,
+ * [n_roots][max_nodes] arrays, node 0 the root.  Expansion k creates the children of the selected leaf at nodes
+ * 1 + 5 k + a.  discount[d] = gamma^d and bound[d] = gamma^d / (1 - gamma) for d in 0..expansions + 1. */
+typedef struct HwyOpdTree {
+    int32_t n_roots, max_nodes, expansions, n_actions;
+    const double *discount, *bound;           /* DEVICE [expansions + 2] */
+    uint8_t *exists, *expanded, *terminal;    /* DEVICE [n_roots][max_nodes] */
+    int32_t *parent, *action, *depth, *branch; /* DEVICE [n_roots][max_nodes]; branch = the root child's action */
+    double *reward, *value, *upper;           /* DEVICE [n_roots][max_nodes] */
+    int32_t *selected;                        /* DEVICE [n_roots][expansions]: the expanded leaf, -1 when none was open */
+    int64_t *leaf_row;                        /* DEVICE [n_roots * n_actions]: store row of the leaf each work row copies */
+    int64_t *recommended;                     /* DEVICE [n_roots] */
+} HwyOpdTree;
+/* Expansion k: (k == 0: reset every tree to its root) select, per root, the open leaf (exists, not expanded, not
+ * terminal) with the largest upper bound, the lowest node on ties; write selected[:, k] and leaf_row[r * n_actions + a]
+ * = r * max_nodes + leaf (the root itself when no leaf is open). */
+int hwy_opd_select(const HwyOpdTree *t, int k, void *stream);
+/* Record the children of expansion k from the work rows r * n_actions + a: available [.][n_actions] u8 (of the leaf's
+ * state), reward f64, terminated / truncated u8 of the step that made them. */
+int hwy_opd_record(const HwyOpdTree *t, int k, const uint8_t *available, const double *reward,
+                   const uint8_t *terminated, const uint8_t *truncated, void *stream);
+/* recommended[r] = the root child action whose subtree holds the largest value (the lowest action on ties). */
+int hwy_opd_recommend(const HwyOpdTree *t, void *stream);
+
 /* Kernel launches issued by the calling thread through this library since load (the
  * `gpu_launches` claim of bench.py). */
 uint64_t hwy_launch_count(void);
