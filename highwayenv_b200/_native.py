@@ -354,26 +354,18 @@ def load():
     lib.hwy_debug_pcg64.restype = C.c_int
     lib.hwy_debug_pcg64.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_int, C.c_void_p]
-    lib.hwy_u_turn_reset.restype = C.c_int
-    lib.hwy_u_turn_reset.argtypes = [NP, NG, C.POINTER(HwyUTurnSpawn), NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_void_p]
-    lib.hwy_two_way_reset.restype = C.c_int
-    lib.hwy_two_way_reset.argtypes = [NP, NG, C.POINTER(HwyTwoWaySpawn), NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                      C.c_void_p]
-    lib.hwy_exit_reset.restype = C.c_int
-    lib.hwy_exit_reset.argtypes = [NP, NG, C.POINTER(HwyExitSpawn), NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p]
-    lib.hwy_merge_reset.restype = C.c_int
-    lib.hwy_merge_reset.argtypes = [NP, NG, C.POINTER(HwyMergeSpawn), NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                    C.c_void_p]
+    # the scripted resets: (params, graph, spawn, state, rng, mask_a, mask_b, obs, stream)
+    for name, spawn in (("hwy_roundabout_reset", HwyRoundaboutSpawn), ("hwy_merge_reset", HwyMergeSpawn),
+                        ("hwy_exit_reset", HwyExitSpawn), ("hwy_u_turn_reset", HwyUTurnSpawn),
+                        ("hwy_two_way_reset", HwyTwoWaySpawn)):
+        fn = getattr(lib, name)
+        fn.restype = C.c_int
+        fn.argtypes = [NP, NG, C.POINTER(spawn), NS] + [C.c_void_p] * 5
     lib.hwy_intersection_reset.restype = C.c_int
     lib.hwy_intersection_reset.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_network_substeps.restype = C.c_int
     lib.hwy_network_substeps.argtypes = [NP, NG, NS, C.c_void_p, C.c_int, C.c_void_p]
-    lib.hwy_roundabout_reset.restype = C.c_int
-    lib.hwy_roundabout_reset.argtypes = [NP, NG, C.POINTER(HwyRoundaboutSpawn), NS, C.c_void_p, C.c_void_p,
-                                         C.c_void_p, C.c_void_p, C.c_void_p]
     OV = C.POINTER(HwyObsView)
     lib.hwy_observe_grid.restype = C.c_int
     lib.hwy_observe_grid.argtypes = [NG, OV, C.POINTER(HwyGridParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

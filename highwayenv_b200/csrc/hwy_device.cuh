@@ -9,6 +9,11 @@ namespace hwy {
 
 typedef unsigned long long u64;
 
+// env e takes part in a masked launch: one of the two masks selects it, or there is no mask at all
+__device__ __forceinline__ bool env_selected(const uint8_t* mask_a, const uint8_t* mask_b, int e) {
+    return (!mask_a && !mask_b) || (mask_a && mask_a[e]) || (mask_b && mask_b[e]);
+}
+
 // ------------------------------------------------------------------ lane geometry
 // road/lane.py:205-209 StraightLane.local_coordinates
 __device__ __forceinline__ void lane_local(const HwyStraightLane& L, double x, double y, double& s,

@@ -1234,7 +1234,7 @@ template <int TPE>
 __global__ void __launch_bounds__(TPE == 32 ? 128 : TPE)
 highway_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                        const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b,
-                       int use_mask, float* __restrict__ obs) {
+                       float* __restrict__ obs) {
     constexpr int EPB = TPE == 32 ? 4 : 1;
     __shared__ ObsShared<TPE> smem[EPB];
     const int sub = threadIdx.x / TPE, i = threadIdx.x % TPE;
@@ -1247,7 +1247,7 @@ highway_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHigh
     load_vehicle(S, (size_t)e * S.vp + (active ? i : 0), r);
     publish(P, sm.f, i, active, r);
     env_sync<TPE>();
-    const bool wanted = env_ok && (!use_mask || (mask_a && mask_a[e]) || (mask_b && mask_b[e]));
+    const bool wanted = env_ok && env_selected(mask_a, mask_b, e);
     kinematics_observe(P, sm.f, sm.key, i, r.heading,
                        wanted ? obs + (size_t)e * P.obs_vehicles_count * obs_columns(P) : nullptr);
 }
@@ -1260,8 +1260,7 @@ highway_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHigh
 // LINEAR: LinearVehicle.randomize_behavior (behavior.py:406-415) draws the traffic's parameters into T->params.
 __global__ void __launch_bounds__(128)
 highway_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
-                     const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b,
-                     int use_mask) {
+                     const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
     constexpr bool LINEAR = false;
     const HwyLinearTraffic* T = nullptr;
 #include "hwy_highway_reset.cuh"
@@ -1270,7 +1269,7 @@ highway_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwa
 __global__ void __launch_bounds__(128)
 highway_linear_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                             const __grid_constant__ HwyLinearTraffic T_, const uint8_t* __restrict__ mask_a,
-                            const uint8_t* __restrict__ mask_b, int use_mask) {
+                            const uint8_t* __restrict__ mask_b) {
     constexpr bool LINEAR = true;
     const HwyLinearTraffic* T = &T_;
 #include "hwy_highway_reset.cuh"
@@ -1329,14 +1328,7 @@ __global__ void debug_pcg64_kernel(int op, int arg_i, double arg_lo, double arg_
                                    uint64_t* __restrict__ draws, int n) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n) return;
-    Pcg64 g;
-    g.s_hi = words_in[0 * (size_t)n + e];
-    g.s_lo = words_in[1 * (size_t)n + e];
-    g.i_hi = words_in[2 * (size_t)n + e];
-    g.i_lo = words_in[3 * (size_t)n + e];
-    const uint64_t w4 = words_in[4 * (size_t)n + e];
-    g.has32 = (uint32_t)(w4 >> 32);
-    g.u32 = (uint32_t)w4;
+    Pcg64 g = load_rng(words_in, (size_t)n, e);
     if (op == HWY_PCG_AT) {
         g = pcg_at(g, arg_i);
     } else {
@@ -1363,11 +1355,7 @@ __global__ void debug_pcg64_kernel(int op, int arg_i, double arg_lo, double arg_
             }
         }
     }
-    words_out[0 * (size_t)n + e] = g.s_hi;
-    words_out[1 * (size_t)n + e] = g.s_lo;
-    words_out[2 * (size_t)n + e] = g.i_hi;
-    words_out[3 * (size_t)n + e] = g.i_lo;
-    words_out[4 * (size_t)n + e] = ((uint64_t)g.has32 << 32) | g.u32;
+    store_rng_all(words_out, (size_t)n, e, g);
 }
 
 }  // namespace hwy
@@ -1576,29 +1564,29 @@ int launch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLi
 }
 
 int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask_a,
-                   const uint8_t* mask_b, int use_mask, float* obs, cudaStream_t st) {
+                   const uint8_t* mask_b, float* obs, cudaStream_t st) {
     int tpe = tpe_for(p->n_vehicles);
     Grid g = grid_for(tpe, s->n_envs);
     if (tpe == 32)
-        hwy::highway_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, use_mask, obs);
+        hwy::highway_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
     else if (tpe == 64)
-        hwy::highway_observe_kernel<64><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, use_mask, obs);
+        hwy::highway_observe_kernel<64><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
     else
-        hwy::highway_observe_kernel<128><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, use_mask, obs);
+        hwy::highway_observe_kernel<128><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
     return check_launch("highway_observe_kernel");
 }
 
 int launch_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask_a,
-                 const uint8_t* mask_b, int use_mask, cudaStream_t st) {
+                 const uint8_t* mask_b, cudaStream_t st) {
     int blocks = (s->n_envs + 127) / 128;
-    hwy::highway_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, mask_a, mask_b, use_mask);
+    hwy::highway_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, mask_a, mask_b);
     return check_launch("highway_reset_kernel");
 }
 
 int launch_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                        const uint8_t* mask_a, const uint8_t* mask_b, int use_mask, cudaStream_t st) {
+                        const uint8_t* mask_a, const uint8_t* mask_b, cudaStream_t st) {
     int blocks = (s->n_envs + 127) / 128;
-    hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b, use_mask);
+    hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b);
     return check_launch("highway_linear_reset_kernel");
 }
 
@@ -1628,17 +1616,16 @@ int hwy_highway_slot_stride(int n_vehicles) { return (n_vehicles + 1) & ~1; }
 int hwy_highway_observe(const HwyHighwayParams* p, const HwyHighwayState* s, float* obs, void* stream) {
     if (validate(p, s)) return 1;
     if (!obs) return fail("%s", "obs is null");
-    return launch_observe(p, s, nullptr, nullptr, 0, obs, (cudaStream_t)stream);
+    return launch_observe(p, s, nullptr, nullptr, obs, (cudaStream_t)stream);
 }
 
 int hwy_highway_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask,
                       float* obs, void* stream) {
     if (validate(p, s)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
-    int use_mask = mask != nullptr;
     if (ensure_pcg_jump(st)) return 1;  // the fused autoreset of later steps reads the table
-    if (launch_reset(p, s, mask, nullptr, use_mask, st)) return 1;
-    if (obs) return launch_observe(p, s, mask, nullptr, use_mask, obs, st);
+    if (launch_reset(p, s, mask, nullptr, st)) return 1;
+    if (obs) return launch_observe(p, s, mask, nullptr, obs, st);
     return 0;
 }
 
@@ -1688,8 +1675,8 @@ int hwy_highway_autoreset(const HwyHighwayParams* p, const HwyHighwayState* s,
     if (validate(p, s)) return 1;
     if (!terminated || !truncated || !obs) return fail("%s", "null pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    if (launch_reset(p, s, terminated, truncated, 1, st)) return 1;
-    return launch_observe(p, s, terminated, truncated, 1, obs, st);
+    if (launch_reset(p, s, terminated, truncated, st)) return 1;
+    return launch_observe(p, s, terminated, truncated, obs, st);
 }
 
 int hwy_highway_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
@@ -1715,10 +1702,9 @@ int hwy_highway_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s
                              const uint8_t* mask, float* obs, void* stream) {
     if (validate(p, s) || validate_linear(t)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
-    int use_mask = mask != nullptr;
     if (ensure_pcg_jump(st)) return 1;
-    if (launch_linear_reset(p, s, t, mask, nullptr, use_mask, st)) return 1;
-    if (obs) return launch_observe(p, s, mask, nullptr, use_mask, obs, st);
+    if (launch_linear_reset(p, s, t, mask, nullptr, st)) return 1;
+    if (obs) return launch_observe(p, s, mask, nullptr, obs, st);
     return 0;
 }
 
@@ -1727,8 +1713,8 @@ int hwy_highway_linear_autoreset(const HwyHighwayParams* p, const HwyHighwayStat
     if (validate(p, s) || validate_linear(t)) return 1;
     if (!terminated || !truncated || !obs) return fail("%s", "null pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    if (launch_linear_reset(p, s, t, terminated, truncated, 1, st)) return 1;
-    return launch_observe(p, s, terminated, truncated, 1, obs, st);
+    if (launch_linear_reset(p, s, t, terminated, truncated, st)) return 1;
+    return launch_observe(p, s, terminated, truncated, obs, st);
 }
 
 int hwy_highway_linear_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,

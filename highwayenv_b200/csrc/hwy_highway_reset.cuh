@@ -2,17 +2,8 @@
 // and highway_linear_reset_kernel (LINEAR = true) in hwy_highway.cu.  In scope: LINEAR, the kernel parameters and
 // `const HwyLinearTraffic* T`.
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if (use_mask && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
-    const int n = S.n_envs;
-    Pcg64 g;
-    g.s_hi = S.rng[0 * (size_t)n + e];
-    g.s_lo = S.rng[1 * (size_t)n + e];
-    g.i_hi = S.rng[2 * (size_t)n + e];
-    g.i_lo = S.rng[3 * (size_t)n + e];
-    u64 w4 = S.rng[4 * (size_t)n + e];
-    g.has32 = (uint32_t)(w4 >> 32);
-    g.u32 = (uint32_t)w4;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
+    Pcg64 g = load_rng(S.rng, (size_t)S.n_envs, e);
 
     double x_max = 0.0;  // running max of the longitudinal coordinates of spawned vehicles
     bool aligned = true;  // all lanes share origin-x and direction => s is lane independent
@@ -87,8 +78,4 @@
     }
     S.speed_index[e] = ego_speed_index;
     S.time[e] = 0.0;
-    S.rng[0 * (size_t)n + e] = g.s_hi;
-    S.rng[1 * (size_t)n + e] = g.s_lo;
-    S.rng[2 * (size_t)n + e] = g.i_hi;
-    S.rng[3 * (size_t)n + e] = g.i_lo;
-    S.rng[4 * (size_t)n + e] = ((u64)g.has32 << 32) | g.u32;
+    store_rng_all(S.rng, (size_t)S.n_envs, e, g);

@@ -245,4 +245,30 @@ struct Pcg64 {
     }
 };
 
+// The stream words of env e in a [5][n] table (HwyHighwayState.rng, HwyNetState.rng): state hi / lo, increment
+// hi / lo, has32 << 32 | u32.
+__device__ __forceinline__ Pcg64 load_rng(const uint64_t* rng, size_t n, int e) {
+    Pcg64 g;
+    g.s_hi = rng[0 * n + e];
+    g.s_lo = rng[1 * n + e];
+    g.i_hi = rng[2 * n + e];
+    g.i_lo = rng[3 * n + e];
+    uint64_t w4 = rng[4 * n + e];
+    g.has32 = (uint32_t)(w4 >> 32);
+    g.u32 = (uint32_t)w4;
+    return g;
+}
+// the words a draw changes: the state and the buffered 32-bit half (the increment is constant)
+__device__ __forceinline__ void store_rng(uint64_t* rng, size_t n, int e, const Pcg64& g) {
+    rng[0 * n + e] = g.s_hi;
+    rng[1 * n + e] = g.s_lo;
+    rng[4 * n + e] = ((uint64_t)g.has32 << 32) | g.u32;
+}
+// all five words
+__device__ __forceinline__ void store_rng_all(uint64_t* rng, size_t n, int e, const Pcg64& g) {
+    store_rng(rng, n, e, g);
+    rng[2 * n + e] = g.i_hi;
+    rng[3 * n + e] = g.i_lo;
+}
+
 }  // namespace hwy

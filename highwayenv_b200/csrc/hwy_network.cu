@@ -19,7 +19,6 @@
 // Reference paths are relative to /root/reference/highway_env.
 #include <atomic>
 #include <cstdio>
-#include <cstdlib>
 #include <mutex>
 
 #include <cuda_runtime.h>
@@ -1521,23 +1520,6 @@ __device__ __forceinline__ void adopt_spawn(const HwyNetParams& P, const HwyInte
     publish(st, i, r);
 }
 
-__device__ __forceinline__ Pcg64 load_rng(const uint64_t* rng, size_t n, int e) {
-    Pcg64 g;
-    g.s_hi = rng[0 * n + e];
-    g.s_lo = rng[1 * n + e];
-    g.i_hi = rng[2 * n + e];
-    g.i_lo = rng[3 * n + e];
-    uint64_t w4 = rng[4 * n + e];
-    g.has32 = (uint32_t)(w4 >> 32);
-    g.u32 = (uint32_t)w4;
-    return g;
-}
-__device__ __forceinline__ void store_rng(uint64_t* rng, size_t n, int e, const Pcg64& g) {
-    rng[0 * n + e] = g.s_hi;
-    rng[1 * n + e] = g.s_lo;
-    rng[4 * n + e] = ((uint64_t)g.has32 << 32) | g.u32;
-}
-
 // ------------------------------------------------------------------ the step kernel
 template <int G, bool REG, bool PLAIN>
 __global__ void __launch_bounds__(kStepThreads, 1)
@@ -1814,8 +1796,7 @@ network_observe_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph
     EnvStage<G, REG>& st = stages[sub];
     Regs r;
     load_env(P, g, S, st, e, i, r);
-    const bool selected = (!mask_a && !mask_b) || (mask_a && mask_a[e]) || (mask_b && mask_b[e]);
-    if (!selected) return;  // whole group leaves together (selection is per env)
+    if (!env_selected(mask_a, mask_b, e)) return;  // whole group leaves together (selection is per env)
     observe_agents(P, g, st, i, obs + (size_t)e * n_agents_of(P) * obs_size(P));
 }
 
@@ -1892,7 +1873,7 @@ network_substeps_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
 __global__ void compact_envs_kernel(const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b, int n_envs,
                                     int* __restrict__ list) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool sel = e < n_envs && ((!mask_a && !mask_b) || (mask_a && mask_a[e]) || (mask_b && mask_b[e]));
+    const bool sel = e < n_envs && env_selected(mask_a, mask_b, e);
     const unsigned m = __ballot_sync(0xffffffffu, sel);
     if (!m) return;
     const int lane = threadIdx.x & 31;
@@ -1934,8 +1915,6 @@ intersection_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGr
     GraphShared& g = *reinterpret_cast<GraphShared*>(smem_raw);
     EnvStage<G, REG>* stages =
         reinterpret_cast<EnvStage<G, REG>*>(smem_raw + ((sizeof(GraphShared) + 15) & ~size_t(15)));
-    // The reset is a long dependent chain per env (9 spawn attempts, 45 warm-up substeps, ...) for the few envs that
-    // ended (~8 % per step): small blocks (kResetThreads) spread them over all SMs and shorten the lock-step waits.
     const int kEnvs = blockDim.x / G;
     const int n_sel = list[0];
     if (blockIdx.x * kEnvs >= n_sel) return;  // uniform per block
@@ -2049,6 +2028,51 @@ intersection_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGr
     observe_agents(P, g, st, i, obs + (size_t)e * A * obs_size(P));
 }
 
+// ------------------------------------------------------------------ the scripted resets
+// The _make_vehicles of roundabout, merge, exit, u-turn and two-way: a fixed placement drawn from the env's numpy
+// stream, for the envs the masks select.  Each family kernel keeps its own placement and draw order; the helpers
+// below are the rest.
+
+// RoadObject.__init__ (objects.py:46-50): the closest lane, first minimum in graph-enumeration order
+__device__ __forceinline__ int closest_lane(const HwyNetGraph* graph, double x, double y, double heading) {
+    int lane = 0;
+    double bd = 0;
+    for (int l = 0; l < graph->n_lanes; ++l) {
+        const double d = lane_distance_with_heading(graph->lanes[l], x, y, heading);
+        if (l == 0 || d < bd) {
+            bd = d;
+            lane = l;
+        }
+    }
+    return lane;
+}
+
+// One placed vehicle into slot k, with no impact; IDM vehicles get IDMVehicle.__init__'s lane-change timer
+// (behavior.py:64).  `flags`: further meta bits (HWY_META_NO_LANE_CHANGE).
+__device__ __forceinline__ void store_vehicle(const HwyNetParams& P, const HwyNetState& S, size_t k, double px,
+                                              double py, double heading, double speed, double target_speed,
+                                              double delta, int lane, int target, int kind, int flags = 0) {
+    const double timer = kind == HWY_KIND_IDM ? py_mod_pos((px + py) * kPi, P.lane_change_delay) : 0.0;
+    reinterpret_cast<double2*>(S.pos)[k] = make_double2(px, py);
+    reinterpret_cast<double2*>(S.hs)[k] = make_double2(heading, speed);
+    reinterpret_cast<double2*>(S.tt)[k] = make_double2(target_speed, timer);
+    reinterpret_cast<double2*>(S.imp)[k] = make_double2(0.0, 0.0);
+    S.delta[k] = delta;
+    S.meta[k] = (lane << HWY_META_LANE_SHIFT) | (target << HWY_META_TARGET_SHIFT) | HWY_META_CHECK_COLLISIONS |
+                (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT | flags;
+}
+
+// The per-env end of a scripted reset: the ego's speed index, the clock, the advanced stream, and the population
+// and RegulatedRoad clock where the state has them (the 32-slot state of exit-v0)
+__device__ __forceinline__ void store_env_tail(const HwyNetState& S, uint64_t* rng, int e, int speed_index, int count,
+                                               const Pcg64& g) {
+    S.speed_index[e] = speed_index;
+    S.time[e] = 0.0;
+    if (S.count) S.count[e] = count;
+    if (S.road_steps) S.road_steps[e] = 0;
+    store_rng(rng, (size_t)S.n_envs, e, g);
+}
+
 // RoundaboutEnv._make_vehicles (envs/roundabout_env.py:317-391), one env per WARP.  The draws are a sequential chain
 // on the env's numpy stream: every lane of the warp walks it redundantly (same instructions, same values — no
 // shuffles), and the expensive part, RoadObject.__init__'s closest-lane search over all 32 lanes of the network for
@@ -2061,24 +2085,10 @@ roundabout_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
                         const uint8_t* __restrict__ mask_b) {
     const int e = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const int wl = threadIdx.x & 31;
-    if (e >= S.n_envs) return;  // warp-uniform
-    if ((mask_a || mask_b) && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
-    const size_t n = (size_t)S.n_envs;
-    Pcg64 g;
-    g.s_hi = rng[0 * n + e];
-    g.s_lo = rng[1 * n + e];
-    g.i_hi = rng[2 * n + e];
-    g.i_lo = rng[3 * n + e];
-    uint64_t w4 = rng[4 * n + e];
-    g.has32 = (uint32_t)(w4 >> 32);
-    g.u32 = (uint32_t)w4;
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;  // warp-uniform
+    Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
     const size_t base = (size_t)e * S.vp;
-    const int V = P.n_vehicles;
-    for (int v = 0; v < V; ++v) {
+    for (int v = 0; v < P.n_vehicles; ++v) {
         const bool is_ego = v == 0;
         double px, py, heading, speed, delta = 4.0;
         int dest = 3;
@@ -2097,7 +2107,7 @@ roundabout_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
             lane_position(L, lon, 0.0, px, py);  // make_on_lane (vehicle/objects.py:68-90)
             heading = lane_heading_at(L, lon);
         }
-        // RoadObject.__init__: closest lane (objects.py:46-50), first minimum in graph-enumeration order
+        // closest_lane over the warp
         double bd = INFINITY;
         int lane = 0x7fffffff;
         for (int l = wl; l < graph->n_lanes; l += 32) {
@@ -2116,35 +2126,16 @@ roundabout_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
                 lane = l2;
             }
         }
-        double target_speed = speed, timer = 0.0;
-        int kind = HWY_KIND_IDM;
-        if (is_ego) {
-            kind = HWY_KIND_MDP;
-            target_speed = P.target_speeds[SP.ego_speed_index];
-        } else {
-            timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
-        }
         if (wl == 0) {
-            pos[base + v] = make_double2(px, py);
-            hs[base + v] = make_double2(heading, speed);
-            tt[base + v] = make_double2(target_speed, timer);
-            imp[base + v] = make_double2(0.0, 0.0);
-            S.delta[base + v] = delta;
-            S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) |
-                               HWY_META_CHECK_COLLISIONS | (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT;
+            store_vehicle(P, S, base + v, px, py, heading, speed, is_ego ? P.target_speeds[SP.ego_speed_index] : speed,
+                          delta, lane, lane, is_ego ? HWY_KIND_MDP : HWY_KIND_IDM);
             S.route_len[base + v] = SP.route_len[(size_t)lane * 4 + dest];
         }
         const int* rsrc = SP.route_table + ((size_t)lane * 4 + dest) * R;
         int* rdst = S.route + (base + v) * R;
         for (int k = wl; k < R; k += 32) rdst[k] = rsrc[k];
     }
-    if (wl == 0) {
-        S.speed_index[e] = SP.ego_speed_index;
-        S.time[e] = 0.0;
-        rng[0 * n + e] = g.s_hi;
-        rng[1 * n + e] = g.s_lo;
-        rng[4 * n + e] = ((uint64_t)g.has32 << 32) | g.u32;
-    }
+    if (wl == 0) store_env_tail(S, rng, e, SP.ego_speed_index, P.n_vehicles, g);
 }
 
 // MergeEnv._make_vehicles and the ramp's Obstacle (envs/merge_env.py:150-190), one env per thread
@@ -2153,17 +2144,12 @@ merge_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __
                    const __grid_constant__ HwyMergeSpawn SP, const __grid_constant__ HwyNetState S,
                    uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if ((mask_a || mask_b) && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
     Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
     const size_t base = (size_t)e * S.vp;
     const double base_position[3] = {90.0, 70.0, 5.0}, base_speed[3] = {29.0, 31.0, 31.5};
     for (int v = 0; v < 6; ++v) {
-        double px, py, speed, target_speed, timer = 0.0;
+        double px, py, speed, target_speed;
         int kind = HWY_KIND_IDM;
         if (v == 0) {  // :158-161 ego = action_type.vehicle_class(road, ("a","b",1).position(30, 0), speed=30)
             lane_position(graph->lanes[SP.lane_ab[1]], 30.0, 0.0, px, py);
@@ -2185,28 +2171,12 @@ merge_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __
             speed = target_speed = 0.0;
             kind = HWY_KIND_OBSTACLE;
         }
-        int lane = 0;  // RoadObject.__init__: closest lane at heading 0 (objects.py:46-50)
-        double bd = 0;
-        for (int l = 0; l < graph->n_lanes; ++l) {
-            double d = lane_distance_with_heading(graph->lanes[l], px, py, 0.0);
-            if (l == 0 || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
-        if (kind == HWY_KIND_IDM) timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
-        pos[base + v] = make_double2(px, py);
-        hs[base + v] = make_double2(0.0, speed);
-        tt[base + v] = make_double2(target_speed, timer);
-        imp[base + v] = make_double2(0.0, 0.0);
-        S.delta[base + v] = 4.0;  // IDMVehicle.DELTA: randomize_behavior is not called here
-        S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) | HWY_META_CHECK_COLLISIONS |
-                           (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT;
+        const int lane = closest_lane(graph, px, py, 0.0);  // at heading 0
+        // DELTA 4: randomize_behavior is not called here
+        store_vehicle(P, S, base + v, px, py, 0.0, speed, target_speed, 4.0, lane, lane, kind);
         S.route_len[base + v] = 0;
     }
-    S.speed_index[e] = SP.ego_speed_index;
-    S.time[e] = 0.0;
-    store_rng(rng, (size_t)S.n_envs, e, g);
+    store_env_tail(S, rng, e, SP.ego_speed_index, P.n_vehicles, g);
 }
 
 // ExitEnv._create_vehicles (envs/exit_env.py:107-145), one env per thread (the longitudinal positions are a running
@@ -2218,13 +2188,8 @@ exit_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __r
                   const __grid_constant__ HwyExitSpawn SP, const __grid_constant__ HwyNetState S,
                   uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if ((mask_a || mask_b) && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
     Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
     const size_t base = (size_t)e * S.vp;
     double x_max = 0.0;
     for (int v = 0; v < SP.n_vehicles; ++v) {
@@ -2248,44 +2213,23 @@ exit_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __r
         const double heading = L.heading;
         const double s_here = lane_s_of(graph->lanes[0], px, py);
         x_max = v == 0 ? s_here : fmax(x_max, s_here);
-        int lane = 0;  // RoadObject.__init__: closest lane (objects.py:46-50)
-        double bd = 0;
-        for (int l = 0; l < graph->n_lanes; ++l) {
-            double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
-            if (l == 0 || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
-        double target_speed = speed, timer = 0.0;
-        int kind = HWY_KIND_IDM, extra = HWY_META_NO_LANE_CHANGE;  // vehicle.enable_lane_change = False (:143)
-        int* route = S.route + (base + v) * R;
+        const int lane = closest_lane(graph, px, py, heading);
         if (is_ego) {  // MDPVehicle.__init__ (controller.py:283-293); no route
-            kind = HWY_KIND_MDP;
-            extra = 0;
-            target_speed = P.target_speeds[SP.ego_speed_index];
+            store_vehicle(P, S, base + v, px, py, heading, speed, P.target_speeds[SP.ego_speed_index], 4.0, lane, lane,
+                          HWY_KIND_MDP);
             S.route_len[base + v] = 0;
-        } else {
-            timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
+        } else {  // vehicle.enable_lane_change = False (:143)
+            store_vehicle(P, S, base + v, px, py, heading, speed, speed, 4.0, lane, lane, HWY_KIND_IDM,
+                          HWY_META_NO_LANE_CHANGE);
             const HwyNetLane& CL = graph->lanes[lane];  // plan_route_to("3") (controller.py:71-87)
+            int* route = S.route + (base + v) * R;
             route[0] = CL.from_node | (CL.to_node << 8) | ((CL.lane_id + 1) << 16);
             route[1] = SP.route_12;
             route[2] = SP.route_23;
             S.route_len[base + v] = 3;
         }
-        pos[base + v] = make_double2(px, py);
-        hs[base + v] = make_double2(heading, speed);
-        tt[base + v] = make_double2(target_speed, timer);
-        imp[base + v] = make_double2(0.0, 0.0);
-        S.delta[base + v] = 4.0;
-        S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) | HWY_META_CHECK_COLLISIONS |
-                           (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT | extra;
     }
-    S.speed_index[e] = SP.ego_speed_index;
-    S.time[e] = 0.0;
-    if (S.count) S.count[e] = SP.n_vehicles;
-    if (S.road_steps) S.road_steps[e] = 0;
-    store_rng(rng, (size_t)S.n_envs, e, g);
+    store_env_tail(S, rng, e, SP.ego_speed_index, SP.n_vehicles, g);
 }
 
 // UTurnEnv._make_vehicles (envs/u_turn_env.py:179-275), one env per thread: the MDPVehicle at the start of
@@ -2295,16 +2239,11 @@ u_turn_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* _
                     const __grid_constant__ HwyUTurnSpawn SP, const __grid_constant__ HwyNetState S,
                     uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if ((mask_a || mask_b) && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
     Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
     const size_t base = (size_t)e * S.vp;
     for (int v = 0; v < 7; ++v) {
-        double px, py, heading, speed, target_speed, timer = 0.0, delta = 4.0;
+        double px, py, heading, speed, target_speed, delta = 4.0;
         int kind = HWY_KIND_IDM;
         if (v == 0) {  // :189-201 ego = vehicle_class(road, ("a","b",0).position(0, 0), speed=16)
             lane_position(graph->lanes[SP.lane[0]], 0.0, 0.0, px, py);
@@ -2321,31 +2260,14 @@ u_turn_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* _
             target_speed = speed;
             if (v == 1) delta = g.uniform(3.5, 4.5);  // only vehicle 1 calls randomize_behavior (:218)
         }
-        int lane = 0;  // RoadObject.__init__: closest lane (objects.py:46-50)
-        double bd = 0;
-        for (int l = 0; l < graph->n_lanes; ++l) {
-            double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
-            if (l == 0 || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
-        if (kind == HWY_KIND_IDM) timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
-        pos[base + v] = make_double2(px, py);
-        hs[base + v] = make_double2(heading, speed);
-        tt[base + v] = make_double2(target_speed, timer);
-        imp[base + v] = make_double2(0.0, 0.0);
-        S.delta[base + v] = delta;
-        S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) | HWY_META_CHECK_COLLISIONS |
-                           (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT;
+        const int lane = closest_lane(graph, px, py, heading);
+        store_vehicle(P, S, base + v, px, py, heading, speed, target_speed, delta, lane, lane, kind);
         const int* rsrc = SP.route_table + (size_t)lane * R;  // plan_route_to("d") from the closest lane
         int* rdst = S.route + (base + v) * R;
         for (int k = 0; k < R; ++k) rdst[k] = rsrc[k];
         S.route_len[base + v] = SP.route_len[lane];
     }
-    S.speed_index[e] = SP.ego_speed_index;
-    S.time[e] = 0.0;
-    store_rng(rng, (size_t)S.n_envs, e, g);
+    store_env_tail(S, rng, e, SP.ego_speed_index, P.n_vehicles, g);
 }
 
 // TwoWayEnv._make_vehicles (envs/two_way_env.py:113-158), one env per thread
@@ -2354,16 +2276,11 @@ two_way_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* 
                      const __grid_constant__ HwyTwoWaySpawn SP, const __grid_constant__ HwyNetState S,
                      uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= S.n_envs) return;
-    if ((mask_a || mask_b) && !((mask_a && mask_a[e]) || (mask_b && mask_b[e]))) return;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
     Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
-    double2* pos = reinterpret_cast<double2*>(S.pos);
-    double2* hs = reinterpret_cast<double2*>(S.hs);
-    double2* tt = reinterpret_cast<double2*>(S.tt);
-    double2* imp = reinterpret_cast<double2*>(S.imp);
     const size_t base = (size_t)e * S.vp;
     for (int v = 0; v < 6; ++v) {
-        double px, py, heading, speed, target_speed, timer = 0.0;
+        double px, py, heading, speed, target_speed;
         int kind = HWY_KIND_IDM, flags = HWY_META_NO_LANE_CHANGE;
         if (v == 0) {  // :120-123 ego on ("a","b",1) at s = 30, speed 30
             const HwyNetLane& L = graph->lanes[SP.lane_ab1];
@@ -2388,29 +2305,12 @@ two_way_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* 
             speed = 20.0 + 5.0 * g.normal();
             target_speed = speed;
         }
-        int lane = 0;  // RoadObject.__init__: closest lane (objects.py:46-50)
-        double bd = 0;
-        for (int l = 0; l < graph->n_lanes; ++l) {
-            double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
-            if (l == 0 || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
+        const int lane = closest_lane(graph, px, py, heading);
         const int target = v >= 4 ? SP.lane_ba0 : lane;  // :157 v.target_lane_index = ("b", "a", 0)
-        if (kind == HWY_KIND_IDM) timer = py_mod_pos((px + py) * kPi, P.lane_change_delay);  // behavior.py:64
-        pos[base + v] = make_double2(px, py);
-        hs[base + v] = make_double2(heading, speed);
-        tt[base + v] = make_double2(target_speed, timer);
-        imp[base + v] = make_double2(0.0, 0.0);
-        S.delta[base + v] = 4.0;
-        S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (target << HWY_META_TARGET_SHIFT) | HWY_META_CHECK_COLLISIONS |
-                           (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT | flags;
+        store_vehicle(P, S, base + v, px, py, heading, speed, target_speed, 4.0, lane, target, kind, flags);
         S.route_len[base + v] = 0;
     }
-    S.speed_index[e] = SP.ego_speed_index;
-    S.time[e] = 0.0;
-    store_rng(rng, (size_t)S.n_envs, e, g);
+    store_env_tail(S, rng, e, SP.ego_speed_index, P.n_vehicles, g);
 }
 
 }  // namespace hwynet
@@ -2475,10 +2375,10 @@ SideStream* side_stream() {
     return table[dev];
 }
 
+// Dynamic shared memory of a block of `per` envs on G slots: the staged lane table, then one EnvStage per env
 template <int G, bool REG>
-size_t net_smem_bytes() {
-    return ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) +
-           (hwynet::kBlockThreads / G) * sizeof(hwynet::EnvStage<G, REG>);
+size_t stage_smem_bytes(int per) {
+    return ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) + (size_t)per * sizeof(hwynet::EnvStage<G, REG>);
 }
 template <typename K>
 int configure_smem(K kernel, size_t bytes) {
@@ -2486,15 +2386,6 @@ int configure_smem(K kernel, size_t bytes) {
     if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
     return 0;
 }
-int reset_threads() {  // HWYB200_RESET_THREADS overrides (32 / 64 / 128 / 256)
-    if (const char* e = getenv("HWYB200_RESET_THREADS")) {
-        int v = atoi(e);
-        if (v == 32 || v == 64 || v == 128 || v == 256) return v;
-    }
-    return 64;
-}
-const int kResetThreads = reset_threads();
-const bool kResetWide = getenv("HWYB200_RESET_WIDE") != nullptr;  // experiment: one env per warp in the reset kernel
 int blocks_for(int n_envs, int g) {
     int per = hwynet::kBlockThreads / g;
     return (n_envs + per - 1) / per;
@@ -2521,19 +2412,9 @@ int sm_count() {
 }
 template <int G, bool REG>
 StepPlan step_plan(int n_envs) {
-    static const int forced = [] {  // HWYB200_STEP_THREADS: fixed block size (experiments)
-        const char* e = getenv("HWYB200_STEP_THREADS");
-        const int v = e ? atoi(e) : 0;
-        return (v >= 32 && v <= hwynet::kStepThreads && v % 32 == 0) ? v : 0;
-    }();
     const int per_max = hwynet::kStepThreads / G, sms = sm_count();
-    int per = per_max;
-    if (forced) {
-        per = forced / G > 0 ? forced / G : 1;
-    } else {
-        const int waves = (n_envs + sms * per_max - 1) / (sms * per_max);
-        per = (n_envs + waves * sms - 1) / (waves * sms);
-    }
+    const int waves = (n_envs + sms * per_max - 1) / (sms * per_max);
+    int per = (n_envs + waves * sms - 1) / (waves * sms);
     int threads = ((per * G + 31) / 32) * 32;
     if (threads > hwynet::kStepThreads) threads = hwynet::kStepThreads;
     per = threads / G;
@@ -2541,13 +2422,8 @@ StepPlan step_plan(int n_envs) {
     plan.threads = threads;
     plan.per = per;
     plan.blocks = (n_envs + per - 1) / per;
-    plan.smem = ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) + (size_t)per * sizeof(hwynet::EnvStage<G, REG>);
+    plan.smem = stage_smem_bytes<G, REG>(per);
     return plan;
-}
-template <int G, bool REG>
-size_t step_smem_max() {
-    return ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) +
-           (size_t)(hwynet::kStepThreads / G) * sizeof(hwynet::EnvStage<G, REG>);
 }
 
 template <int G, bool REG>
@@ -2556,9 +2432,10 @@ int launch_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyInters
                 double* info_speed, uint8_t* info_crashed, cudaStream_t st, const int* list = nullptr,
                 double* agents_reward = nullptr, uint8_t* agents_terminated = nullptr) {
     const StepPlan plan = step_plan<G, REG>(s->n_envs);
+    const size_t smem_max = stage_smem_bytes<G, REG>(hwynet::kStepThreads / G);
     if constexpr (REG) {
         if (p->action_type == 1) {  // a ContinuousAction ego (plain Vehicle / BicycleVehicle): its own instantiation
-            if (configure_smem(hwynet::network_step_kernel<G, REG, true>, step_smem_max<G, REG>())) return 1;
+            if (configure_smem(hwynet::network_step_kernel<G, REG, true>, smem_max)) return 1;
             hwynet::network_step_kernel<G, REG, true><<<plan.blocks, plan.threads, plan.smem, st>>>(
                 *p, graph, *s, sp, action, obs, reward, terminated, truncated, info_speed, info_crashed, list,
                 agents_reward, agents_terminated);
@@ -2566,25 +2443,65 @@ int launch_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyInters
         }
     }
     if (p->action_type == 1) return fail("%s", "ContinuousAction is implemented on the intersection family (32-slot state)");
-    if (configure_smem(hwynet::network_step_kernel<G, REG, false>, step_smem_max<G, REG>())) return 1;
+    if (configure_smem(hwynet::network_step_kernel<G, REG, false>, smem_max)) return 1;
     hwynet::network_step_kernel<G, REG, false><<<plan.blocks, plan.threads, plan.smem, st>>>(
         *p, graph, *s, sp, action, obs, reward, terminated, truncated, info_speed, info_crashed, list, agents_reward,
         agents_terminated);
     return check_launch("network_step_kernel");
 }
-template <int G, bool REG>
-int launch_observe(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, const uint8_t* mask_a,
-                   const uint8_t* mask_b, float* obs, cudaStream_t st) {
-    const size_t smem = net_smem_bytes<G, REG>();
-    if (configure_smem(hwynet::network_observe_kernel<G, REG>, smem)) return 1;
-    hwynet::network_observe_kernel<G, REG><<<blocks_for(s->n_envs, G), hwynet::kBlockThreads, smem, st>>>(
-        *p, graph, *s, mask_a, mask_b, obs);
-    return check_launch("network_observe_kernel");
+
+template <int G_, bool REG_>
+struct Slots {
+    static constexpr int G = G_;
+    static constexpr bool REG = REG_;
+};
+// One launch of a 256-thread group kernel (observe, substeps, debug neighbours) on the state's slot stride:
+// kernel_for(Slots<G, REG>{}) names the kernel's <G, REG> instantiation, <8, false> for the 8-slot state and
+// <32, true> for the 32-slot one.
+template <typename KernelFor, typename... Args>
+int launch_groups(KernelFor kernel_for, const char* name, const HwyNetState* s, cudaStream_t st, const Args&... args) {
+    auto launch = [&](auto slots) {
+        using T = decltype(slots);
+        const auto kernel = kernel_for(slots);
+        const size_t smem = stage_smem_bytes<T::G, T::REG>(hwynet::kBlockThreads / T::G);
+        if (configure_smem(kernel, smem)) return 1;
+        kernel<<<blocks_for(s->n_envs, T::G), hwynet::kBlockThreads, smem, st>>>(args...);
+        return check_launch(name);
+    };
+    if (s->vp == HWY_NET_GROUP) return launch(Slots<HWY_NET_GROUP, false>{});
+    return launch(Slots<HWY_NET_GROUP_LARGE, true>{});
 }
 int observe_dispatch(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, const uint8_t* mask_a,
                      const uint8_t* mask_b, float* obs, cudaStream_t st) {
-    if (s->vp == HWY_NET_GROUP) return launch_observe<HWY_NET_GROUP, false>(p, graph, s, mask_a, mask_b, obs, st);
-    return launch_observe<HWY_NET_GROUP_LARGE, true>(p, graph, s, mask_a, mask_b, obs, st);
+    return launch_groups([](auto t) { return hwynet::network_observe_kernel<decltype(t)::G, decltype(t)::REG>; },
+                         "network_observe_kernel", s, st, *p, graph, *s, mask_a, mask_b, obs);
+}
+
+// The reset is a long dependent chain per env (9 spawn attempts, 45 warm-up substeps, ...) for the few envs that
+// ended (~8 % per step): 64-thread blocks (4 envs on 16 slots, 2 on 32) spread them over all SMs and shorten the
+// lock-step waits.
+template <int G>
+int launch_intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
+                              const HwyNetState* s, float* obs, cudaStream_t st) {
+    constexpr int kThreads = 64, per = kThreads / G;
+    const size_t smem = stage_smem_bytes<G, true>(per);
+    if (configure_smem(hwynet::intersection_reset_kernel<G, true>, smem)) return 1;
+    hwynet::intersection_reset_kernel<G, true>
+        <<<(s->n_envs + per - 1) / per, kThreads, smem, st>>>(*p, graph, *s, *spawn, spawn->scratch, obs);
+    return check_launch("intersection_reset_kernel");
+}
+
+// A scripted reset: the family kernel over 128-thread blocks, `threads_per_env` (1, or 32 for roundabout) per env,
+// then the fresh observation of the envs it reset
+template <typename K, typename Spawn>
+int scripted_reset(K kernel, const char* name, int threads_per_env, const HwyNetParams* p, const HwyNetGraph* graph,
+                   const Spawn* spawn, const HwyNetState* s, uint64_t* rng, const uint8_t* mask_a,
+                   const uint8_t* mask_b, float* obs, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    const int per = 128 / threads_per_env;
+    kernel<<<(s->n_envs + per - 1) / per, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
+    if (check_launch(name)) return 1;
+    return obs ? observe_dispatch(p, graph, s, mask_a, mask_b, obs, st) : 0;
 }
 }  // namespace
 
@@ -2679,42 +2596,17 @@ int hwy_intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, cons
         cudaMemcpyAsync(final_obs, obs, (size_t)s->n_envs * hwy_network_obs_size(p) * sizeof(float),
                         cudaMemcpyDeviceToDevice, st);
     if (check_launch("compact_envs_kernel")) return 1;
-    if (spawn->initial_vehicle_count + 1 <= 16 && !kResetWide && kResetThreads >= 32) {  // n-1 draws + challenger + controlled vehicle fit 16 slots
-        const int per = kResetThreads / 16;
-        const size_t smem = ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) + per * sizeof(hwynet::EnvStage<16, true>);
-        if (configure_smem(hwynet::intersection_reset_kernel<16, true>, smem)) return 1;
-        hwynet::intersection_reset_kernel<16, true>
-            <<<(s->n_envs + per - 1) / per, kResetThreads, smem, st>>>(*p, graph, *s, *spawn, spawn->scratch, obs);
-    } else {
-        const int per = kResetThreads / HWY_NET_GROUP_LARGE;
-        const size_t smem = ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) +
-                            per * sizeof(hwynet::EnvStage<HWY_NET_GROUP_LARGE, true>);
-        if (configure_smem(hwynet::intersection_reset_kernel<HWY_NET_GROUP_LARGE, true>, smem)) return 1;
-        hwynet::intersection_reset_kernel<HWY_NET_GROUP_LARGE, true>
-            <<<(s->n_envs + per - 1) / per, kResetThreads, smem, st>>>(*p, graph, *s, *spawn, spawn->scratch, obs);
-    }
-    return check_launch("intersection_reset_kernel");
+    if (spawn->initial_vehicle_count + 1 <= 16)  // n-1 draws + challenger + controlled vehicle fit 16 slots
+        return launch_intersection_reset<16>(p, graph, spawn, s, obs, st);
+    return launch_intersection_reset<HWY_NET_GROUP_LARGE>(p, graph, spawn, s, obs, st);
 }
 
 int hwy_debug_network_neighbours(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s,
                                  const int32_t* query_lane, int32_t* front, int32_t* rear, void* stream) {
     if (validate_net(p, graph, s)) return 1;
     if (!front || !rear) return fail("%s", "null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (s->vp == HWY_NET_GROUP) {
-        const size_t smem = net_smem_bytes<HWY_NET_GROUP, false>();
-        if (configure_smem(hwynet::debug_neighbours_kernel<HWY_NET_GROUP, false>, smem)) return 1;
-        hwynet::debug_neighbours_kernel<HWY_NET_GROUP, false>
-            <<<blocks_for(s->n_envs, HWY_NET_GROUP), hwynet::kBlockThreads, smem, st>>>(*p, graph, *s, query_lane, front,
-                                                                                       rear);
-    } else {
-        const size_t smem = net_smem_bytes<HWY_NET_GROUP_LARGE, true>();
-        if (configure_smem(hwynet::debug_neighbours_kernel<HWY_NET_GROUP_LARGE, true>, smem)) return 1;
-        hwynet::debug_neighbours_kernel<HWY_NET_GROUP_LARGE, true>
-            <<<blocks_for(s->n_envs, HWY_NET_GROUP_LARGE), hwynet::kBlockThreads, smem, st>>>(*p, graph, *s, query_lane,
-                                                                                             front, rear);
-    }
-    return check_launch("debug_neighbours_kernel");
+    return launch_groups([](auto t) { return hwynet::debug_neighbours_kernel<decltype(t)::G, decltype(t)::REG>; },
+                         "debug_neighbours_kernel", s, (cudaStream_t)stream, *p, graph, *s, query_lane, front, rear);
 }
 
 int hwy_debug_rotated_rectangles_intersect(const double* rects, int n, int32_t* out, void* stream) {
@@ -2729,11 +2621,8 @@ int hwy_merge_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyMe
     if (validate_net(p, graph, s)) return 1;
     if (!spawn || !rng) return fail("%s", "null spawn / rng");
     if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "merge-v0: 5 vehicles + 1 obstacle on 8 slots");
-    cudaStream_t st = (cudaStream_t)stream;
-    hwynet::merge_reset_kernel<<<(s->n_envs + 127) / 128, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
-    if (check_launch("merge_reset_kernel")) return 1;
-    if (obs) return observe_dispatch(p, graph, s, mask_a, mask_b, obs, st);
-    return 0;
+    return scripted_reset(hwynet::merge_reset_kernel, "merge_reset_kernel", 1,
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 int hwy_exit_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyExitSpawn* spawn, const HwyNetState* s,
@@ -2743,11 +2632,8 @@ int hwy_exit_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyExi
     if (s->vp != HWY_NET_GROUP_LARGE || spawn->n_vehicles < 1 || spawn->n_vehicles > HWY_NET_GROUP_LARGE)
         return fail("%s", "exit-v0: 1..32 vehicles on 32 slots");
     if (spawn->lanes_count < 1 || spawn->lanes_count > HWY_MAX_LANES) return fail("%s", "lanes_count out of range");
-    cudaStream_t st = (cudaStream_t)stream;
-    hwynet::exit_reset_kernel<<<(s->n_envs + 127) / 128, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
-    if (check_launch("exit_reset_kernel")) return 1;
-    if (obs) return observe_dispatch(p, graph, s, mask_a, mask_b, obs, st);
-    return 0;
+    return scripted_reset(hwynet::exit_reset_kernel, "exit_reset_kernel", 1,
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 int hwy_u_turn_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyUTurnSpawn* spawn, const HwyNetState* s,
@@ -2755,11 +2641,8 @@ int hwy_u_turn_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyU
     if (validate_net(p, graph, s)) return 1;
     if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng / route table");
     if (s->vp != HWY_NET_GROUP || p->n_vehicles != 7) return fail("%s", "u-turn-v0: 7 vehicles on 8 slots");
-    cudaStream_t st = (cudaStream_t)stream;
-    hwynet::u_turn_reset_kernel<<<(s->n_envs + 127) / 128, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
-    if (check_launch("u_turn_reset_kernel")) return 1;
-    if (obs) return observe_dispatch(p, graph, s, mask_a, mask_b, obs, st);
-    return 0;
+    return scripted_reset(hwynet::u_turn_reset_kernel, "u_turn_reset_kernel", 1,
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 int hwy_two_way_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyTwoWaySpawn* spawn, const HwyNetState* s,
@@ -2767,31 +2650,16 @@ int hwy_two_way_reset(const HwyNetParams* p, const HwyNetGraph* graph, const Hwy
     if (validate_net(p, graph, s)) return 1;
     if (!spawn || !rng) return fail("%s", "null spawn / rng");
     if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "two-way-v0: 6 vehicles on 8 slots");
-    cudaStream_t st = (cudaStream_t)stream;
-    hwynet::two_way_reset_kernel<<<(s->n_envs + 127) / 128, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
-    if (check_launch("two_way_reset_kernel")) return 1;
-    if (obs) return observe_dispatch(p, graph, s, mask_a, mask_b, obs, st);
-    return 0;
+    return scripted_reset(hwynet::two_way_reset_kernel, "two_way_reset_kernel", 1,
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 int hwy_network_substeps(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, const uint8_t* mask,
                          int n_substeps, void* stream) {
     if (validate_net(p, graph, s)) return 1;
     if (n_substeps < 0) return fail("%s", "n_substeps < 0");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (s->vp == HWY_NET_GROUP) {
-        const size_t smem = net_smem_bytes<HWY_NET_GROUP, false>();
-        if (configure_smem(hwynet::network_substeps_kernel<HWY_NET_GROUP, false>, smem)) return 1;
-        hwynet::network_substeps_kernel<HWY_NET_GROUP, false>
-            <<<blocks_for(s->n_envs, HWY_NET_GROUP), hwynet::kBlockThreads, smem, st>>>(*p, graph, *s, mask, n_substeps);
-    } else {
-        const size_t smem = net_smem_bytes<HWY_NET_GROUP_LARGE, true>();
-        if (configure_smem(hwynet::network_substeps_kernel<HWY_NET_GROUP_LARGE, true>, smem)) return 1;
-        hwynet::network_substeps_kernel<HWY_NET_GROUP_LARGE, true>
-            <<<blocks_for(s->n_envs, HWY_NET_GROUP_LARGE), hwynet::kBlockThreads, smem, st>>>(*p, graph, *s, mask,
-                                                                                             n_substeps);
-    }
-    return check_launch("network_substeps_kernel");
+    return launch_groups([](auto t) { return hwynet::network_substeps_kernel<decltype(t)::G, decltype(t)::REG>; },
+                         "network_substeps_kernel", s, (cudaStream_t)stream, *p, graph, *s, mask, n_substeps);
 }
 
 int hwy_network_observe(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, float* obs,
@@ -2807,11 +2675,8 @@ int hwy_roundabout_reset(const HwyNetParams* p, const HwyNetGraph* graph, const 
     if (validate_net(p, graph, s)) return 1;
     if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng pointer");
     if (p->n_vehicles != 5 || s->vp != HWY_NET_GROUP) return fail("%s", "roundabout spawn places exactly 5 vehicles in 8 slots");
-    cudaStream_t st = (cudaStream_t)stream;
-    hwynet::roundabout_reset_kernel<<<(s->n_envs + 3) / 4, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);  // a warp per env
-    if (check_launch("roundabout_reset_kernel")) return 1;
-    if (obs) return observe_dispatch(p, graph, s, mask_a, mask_b, obs, st);
-    return 0;
+    return scripted_reset(hwynet::roundabout_reset_kernel, "roundabout_reset_kernel", 32,  // a warp per env
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 }  // extern "C"

@@ -47,9 +47,6 @@ __device__ int find_ego(const HwyObsView& v, int e, int count, int agent) {
     }
     return 0;
 }
-__device__ __forceinline__ bool env_selected(const uint8_t* a, const uint8_t* b, int e) {
-    return (!a && !b) || (a && a[e]) || (b && b[e]);
-}
 
 // Vehicle.to_dict (vehicle/kinematics.py:237-261) relative to the observer; road objects are not in road.vehicles
 __device__ double vehicle_feature(const GraphShared& g, const HwyObsView& view, int e, int slot, const Veh& o,

@@ -188,7 +188,6 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
         p.connected_lanes = int(bool(cfg.get("neighbour_vehicles_connected_lanes", False)))
         self._params = p
         self.single_action_space = Discrete(5)
-        self.spawner = RoundaboutSpawner(self.net, self.config, self.action_type.target_speeds) if self.ENV_ID.startswith("roundabout") else None
         self.observation_space = batch_space(self.single_observation_space, self.num_envs)
         self.action_space = batch_space(self.single_action_space, self.num_envs)
         self.obs_shape = tuple(self.single_observation_space.shape)
@@ -206,7 +205,8 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
 
     def _build_spawn_tables(self) -> None:
         """Host-planned routes for every (closest lane at spawn, destination) pair + spawn constants."""
-        net, sp = self.net, self.spawner
+        net = self.net
+        sp = self.spawner = RoundaboutSpawner(net, self.config, self.action_type.target_speeds)
         self._route_table = torch.from_numpy(sp.routes).to(self.device)
         self._route_table_len = torch.from_numpy(sp.route_lens).to(self.device)
         s = N.HwyRoundaboutSpawn()
