@@ -266,6 +266,15 @@ class HwyOpdTree(C.Structure):
                                              "recommended")])
 
 
+class HwyMctsTree(C.Structure):
+    _fields_ = ([("n_roots", C.c_int32), ("max_nodes", C.c_int32), ("episodes", C.c_int32), ("horizon", C.c_int32),
+                 ("temperature", C.c_double), ("seed", C.c_uint64)]
+                + [(n, C.c_void_p) for n in ("discount", "decision", "exists", "expanded", "parent", "action",
+                                             "child_base", "n_children", "count", "prior", "value", "n_nodes",
+                                             "skipped", "walk_node", "walk_return", "walk_flags", "leaf", "returns",
+                                             "remap", "actions", "recommended")])
+
+
 class HwyLidarParams(C.Structure):
     _fields_ = [("cells", C.c_int32), ("normalize", C.c_int32), ("maximum_range", C.c_double)]
 
@@ -280,7 +289,7 @@ EXPORTS = (
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
     "hwy_value_iteration", "hwy_highway_linear_reset", "hwy_highway_linear_step", "hwy_highway_linear_autoreset",
     "hwy_highway_linear_substeps", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
-    "hwy_opd_recommend",
+    "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -388,6 +397,15 @@ def load():
     lib.hwy_opd_record.argtypes = [OT, C.c_int] + [C.c_void_p] * 5
     lib.hwy_opd_recommend.restype = C.c_int
     lib.hwy_opd_recommend.argtypes = [OT, C.c_void_p]
+    MT = C.POINTER(HwyMctsTree)
+    lib.hwy_mcts_advance.restype = C.c_int
+    lib.hwy_mcts_advance.argtypes = [MT, C.c_int, C.c_int] + [C.c_void_p] * 5
+    lib.hwy_mcts_backup.restype = C.c_int
+    lib.hwy_mcts_backup.argtypes = [MT, C.c_int, C.c_void_p, C.c_void_p]
+    lib.hwy_mcts_recommend.restype = C.c_int
+    lib.hwy_mcts_recommend.argtypes = [MT, C.c_void_p]
+    lib.hwy_mcts_reroot.restype = C.c_int
+    lib.hwy_mcts_reroot.argtypes = [MT, C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

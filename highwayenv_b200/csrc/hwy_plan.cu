@@ -213,6 +213,215 @@ __global__ void __launch_bounds__(kOpdThreads) opd_recommend_kernel(const __grid
     T.recommended[r] = rec;
 }
 
+// ------------------------------------------------------------------ Monte-Carlo tree search
+// One thread per root, tests/mcts_spec.py step for step.  fp64 arithmetic is spelled with _rn intrinsics so that no
+// contraction can round differently from numpy.
+constexpr int kMctsThreads = 128;
+constexpr uint8_t kWalkDone = 1, kWalkRolling = 2;
+constexpr int kIdle = 1;
+
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// mcts_spec.draw: the finaliser chained over (seed, decision, root, episode, depth, purpose)
+__device__ __forceinline__ uint64_t mcts_draw(const HwyMctsTree& T, int r, int e, int d, int purpose) {
+    const uint64_t words[6] = {T.seed, (uint64_t)*T.decision, (uint64_t)r, (uint64_t)e, (uint64_t)d,
+                               (uint64_t)purpose};
+    uint64_t x = 0;
+    for (int k = 0; k < 6; ++k) x = splitmix64(x + 0x9E3779B97F4A7C15ull + words[k]);
+    return x;
+}
+
+// mcts_spec.pick: floor(u * k), u = (x >> 11) 2^-53, exactly ((x >> 11) * k < 2^56)
+__device__ __forceinline__ int mcts_pick(uint64_t x, int k) { return (int)(((x >> 11) * (uint64_t)k) >> 53); }
+
+// the j-th set bit of a 5-bit mask in ascending order
+__device__ __forceinline__ int nth_set(unsigned mask, int j) {
+    for (int a = 0; a < 5; ++a)
+        if (mask >> a & 1u) {
+            if (j == 0) return a;
+            --j;
+        }
+    return kIdle;
+}
+
+__device__ void mcts_clear(const HwyMctsTree& T, size_t row, int start) {
+    for (int c = start; c < T.max_nodes; ++c) {
+        T.exists[row + c] = 0;
+        T.expanded[row + c] = 0;
+        T.parent[row + c] = -1;
+        T.action[row + c] = -1;
+        T.child_base[row + c] = -1;
+        T.n_children[row + c] = 0;
+        T.count[row + c] = 0;
+        T.prior[row + c] = 0.0;
+        T.value[row + c] = 0.0;
+    }
+    if (start == 0) {
+        T.exists[row] = 1;
+        T.prior[row] = 1.0;
+    }
+}
+
+__global__ void __launch_bounds__(kMctsThreads)
+mcts_advance_kernel(const __grid_constant__ HwyMctsTree T, int e, int d, const uint8_t* __restrict__ available,
+                    const double* __restrict__ reward, const uint8_t* __restrict__ terminated,
+                    const uint8_t* __restrict__ truncated) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= T.n_roots) return;
+    const size_t row = (size_t)r * T.max_nodes;
+    int node = 0;
+    double ret = 0.0;
+    uint8_t flags = 0;
+    if (d == 0) {
+        if (e == 0) T.skipped[r] = 0;
+    } else {
+        node = T.walk_node[r];
+        ret = T.walk_return[r];
+        flags = T.walk_flags[r];
+        if (!(flags & kWalkDone)) {
+            ret = __dadd_rn(ret, __dmul_rn(T.discount[d - 1], reward[r]));
+            if (terminated[r] || truncated[r]) flags |= kWalkDone;
+        }
+    }
+    unsigned avail = 0;
+    for (int a = 0; a < 5; ++a) avail |= (available[(size_t)r * 5 + a] ? 1u : 0u) << a;
+    int act = kIdle;
+    if (!(flags & kWalkDone)) {
+        bool descended = false;
+        if (!(flags & kWalkRolling)) {
+            if (T.expanded[row + node]) {  // descent: the best score, exact ties by a draw
+                const int base = T.child_base[row + node];
+                const double tn = __dmul_rn(T.temperature, (double)T.n_children[row + node]);
+                double score[5], best = 0.0;
+                unsigned cand = 0;
+                for (int a = 0; a < 5; ++a) {
+                    const size_t c = row + base + a;
+                    if (!T.exists[c]) continue;
+                    score[a] = __dadd_rn(T.value[c], __ddiv_rn(__dmul_rn(tn, T.prior[c]), (double)(T.count[c] + 1)));
+                    if (!cand || score[a] > best) best = score[a];
+                    cand |= 1u << a;
+                }
+                unsigned ties = 0;
+                for (int a = 0; a < 5; ++a)
+                    if ((cand >> a & 1u) && score[a] == best) ties |= 1u << a;
+                act = nth_set(ties, mcts_pick(mcts_draw(T, r, e, d, 0), __popc(ties)));
+                node = base + act;
+                descended = true;
+            } else {  // expansion of the leaf, unless the tree is full
+                const int base = T.n_nodes[r];
+                if (base + 5 > T.max_nodes) {
+                    T.skipped[r] += 1;
+                } else {
+                    const int k = __popc(avail);
+                    T.n_nodes[r] = base + 5;
+                    T.expanded[row + node] = 1;
+                    T.child_base[row + node] = base;
+                    T.n_children[row + node] = k;
+                    for (int a = 0; a < 5; ++a) {
+                        const size_t c = row + base + a;
+                        const bool ok = avail >> a & 1u;
+                        T.parent[c] = node;
+                        T.action[c] = a;
+                        T.exists[c] = ok;
+                        T.prior[c] = ok ? __ddiv_rn(1.0, (double)k) : 0.0;
+                    }
+                }
+                flags |= kWalkRolling;
+            }
+        }
+        if (!descended) act = nth_set(avail, mcts_pick(mcts_draw(T, r, e, d, 1), __popc(avail)));
+    }
+    T.actions[r] = act;
+    T.walk_node[r] = node;
+    T.walk_return[r] = ret;
+    T.walk_flags[r] = flags;
+}
+
+__global__ void __launch_bounds__(kMctsThreads)
+mcts_backup_kernel(const __grid_constant__ HwyMctsTree T, int e, const double* __restrict__ reward) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= T.n_roots) return;
+    const size_t row = (size_t)r * T.max_nodes;
+    const int node = T.walk_node[r];
+    double ret = T.walk_return[r];
+    // the last step's flags end nothing: only its reward counts
+    if (!(T.walk_flags[r] & kWalkDone)) ret = __dadd_rn(ret, __dmul_rn(T.discount[T.horizon - 1], reward[r]));
+    for (int c = node; c >= 0; c = T.parent[row + c]) {
+        const int n = T.count[row + c] + 1;
+        const double v = T.value[row + c];
+        T.count[row + c] = n;
+        T.value[row + c] = __dadd_rn(v, __dmul_rn(__ddiv_rn(1.0, (double)n), __dsub_rn(ret, v)));
+    }
+    T.leaf[(size_t)r * T.episodes + e] = node;
+    T.returns[(size_t)r * T.episodes + e] = ret;
+}
+
+__global__ void __launch_bounds__(kMctsThreads) mcts_recommend_kernel(const __grid_constant__ HwyMctsTree T) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r == 0) *T.decision += 1;  // no thread of this kernel draws
+    if (r >= T.n_roots) return;
+    const size_t row = (size_t)r * T.max_nodes;
+    int64_t rec = -1;
+    if (T.expanded[row]) {
+        const int base = T.child_base[row];
+        for (int a = 0; a < 5; ++a) {
+            const size_t c = row + base + a;
+            if (!T.exists[c]) continue;
+            const size_t b = row + base + rec;
+            if (rec < 0 || T.count[c] > T.count[b] || (T.count[c] == T.count[b] && T.value[c] > T.value[b])) rec = a;
+        }
+    }
+    T.recommended[r] = rec;
+}
+
+__global__ void __launch_bounds__(kMctsThreads)
+mcts_reroot_kernel(const __grid_constant__ HwyMctsTree T, const int64_t* __restrict__ actions,
+                   const uint8_t* __restrict__ done) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= T.n_roots) return;
+    const size_t row = (size_t)r * T.max_nodes;
+    int c = -1;
+    if (actions && !done[r] && T.expanded[row]) {
+        const int64_t a = actions[r];
+        if (a >= 0 && a < 5 && T.exists[row + T.child_base[row] + a]) c = T.child_base[row] + (int)a;
+    }
+    if (c < 0) {
+        mcts_clear(T, row, 0);
+        T.n_nodes[r] = 1;
+        return;
+    }
+    // the kept slots: c, then every slot whose parent is kept (parents precede children); new indices in order
+    int32_t* remap = T.remap + row;
+    for (int j = 0; j < T.max_nodes; ++j) remap[j] = -1;
+    remap[c] = 0;
+    int k = 1;
+    for (int j = c + 1; j < T.max_nodes; ++j) {
+        const int p = T.parent[row + j];
+        if (p >= 0 && remap[p] >= 0) remap[j] = k++;
+    }
+    for (int j = c; j < T.max_nodes; ++j) {  // remap[j] <= j: in place, ascending
+        const int n = remap[j];
+        if (n < 0) continue;
+        const size_t s = row + j, t = row + n;
+        const int p = T.parent[s], cb = T.child_base[s];
+        T.exists[t] = T.exists[s];
+        T.expanded[t] = T.expanded[s];
+        T.action[t] = T.action[s];
+        T.n_children[t] = T.n_children[s];
+        T.count[t] = T.count[s];
+        T.prior[t] = T.prior[s];
+        T.value[t] = T.value[s];
+        T.parent[t] = j == c ? -1 : remap[p];
+        T.child_base[t] = cb < 0 ? -1 : remap[cb];
+    }
+    mcts_clear(T, row, k);
+    T.n_nodes[r] = k;
+}
+
 }  // namespace hwyplan
 
 // ====================================================================== C ABI
@@ -299,4 +508,53 @@ extern "C" int hwy_opd_recommend(const HwyOpdTree* t, void* stream) {
     if (validate_opd(t)) return 1;
     hwyplan::opd_recommend_kernel<<<opd_blocks(t), hwyplan::kOpdThreads, 0, (cudaStream_t)stream>>>(*t);
     return hwy_abi::check_launch("opd_recommend_kernel");
+}
+
+namespace {
+int validate_mcts(const HwyMctsTree* t) {
+    using hwy_abi::fail;
+    if (!t) return fail("%s", "null tree");
+    if (t->n_roots < 1) return fail("%s", "n_roots must be >= 1");
+    if (t->max_nodes < 6 || (t->max_nodes - 1) % 5 != 0) return fail("%s", "max_nodes must be 1 + 5 k, k >= 1");
+    if (t->episodes < 1 || t->horizon < 1) return fail("%s", "episodes and horizon must be >= 1");
+    if (!(t->temperature >= 0.0 && t->temperature <= 1.7976931348623157e308))
+        return fail("%s", "temperature must be finite and >= 0");
+    if (!t->discount || !t->decision || !t->exists || !t->expanded || !t->parent || !t->action || !t->child_base ||
+        !t->n_children || !t->count || !t->prior || !t->value || !t->n_nodes || !t->skipped || !t->walk_node ||
+        !t->walk_return || !t->walk_flags || !t->leaf || !t->returns || !t->remap || !t->actions || !t->recommended)
+        return fail("%s", "null tree buffer");
+    return 0;
+}
+unsigned mcts_blocks(const HwyMctsTree* t) { return (t->n_roots + hwyplan::kMctsThreads - 1) / hwyplan::kMctsThreads; }
+}  // namespace
+
+extern "C" int hwy_mcts_advance(const HwyMctsTree* t, int e, int d, const uint8_t* available, const double* reward,
+                                const uint8_t* terminated, const uint8_t* truncated, void* stream) {
+    if (validate_mcts(t)) return 1;
+    if (e < 0 || e >= t->episodes || d < 0 || d >= t->horizon) return hwy_abi::fail("%s", "episode or step out of range");
+    if (!available || !reward || !terminated || !truncated) return hwy_abi::fail("%s", "null pointer");
+    hwyplan::mcts_advance_kernel<<<mcts_blocks(t), hwyplan::kMctsThreads, 0, (cudaStream_t)stream>>>(
+        *t, e, d, available, reward, terminated, truncated);
+    return hwy_abi::check_launch("mcts_advance_kernel");
+}
+
+extern "C" int hwy_mcts_backup(const HwyMctsTree* t, int e, const double* reward, void* stream) {
+    if (validate_mcts(t)) return 1;
+    if (e < 0 || e >= t->episodes) return hwy_abi::fail("%s", "episode out of range");
+    if (!reward) return hwy_abi::fail("%s", "null pointer");
+    hwyplan::mcts_backup_kernel<<<mcts_blocks(t), hwyplan::kMctsThreads, 0, (cudaStream_t)stream>>>(*t, e, reward);
+    return hwy_abi::check_launch("mcts_backup_kernel");
+}
+
+extern "C" int hwy_mcts_recommend(const HwyMctsTree* t, void* stream) {
+    if (validate_mcts(t)) return 1;
+    hwyplan::mcts_recommend_kernel<<<mcts_blocks(t), hwyplan::kMctsThreads, 0, (cudaStream_t)stream>>>(*t);
+    return hwy_abi::check_launch("mcts_recommend_kernel");
+}
+
+extern "C" int hwy_mcts_reroot(const HwyMctsTree* t, const int64_t* actions, const uint8_t* done, void* stream) {
+    if (validate_mcts(t)) return 1;
+    if ((actions == nullptr) != (done == nullptr)) return hwy_abi::fail("%s", "actions and done go together");
+    hwyplan::mcts_reroot_kernel<<<mcts_blocks(t), hwyplan::kMctsThreads, 0, (cudaStream_t)stream>>>(*t, actions, done);
+    return hwy_abi::check_launch("mcts_reroot_kernel");
 }

@@ -17,6 +17,14 @@ clones of every env (`env.copy_envs`, csrc/hwy_copy.cu), with its tree kernels i
 
     policy = OpdPolicy(env, budget=50, gamma=0.7)
     env.step(policy.act())
+
+`MctsPolicy` is open-loop Monte-Carlo tree search on the same clones, optionally keeping the subtree of the action
+taken across decisions:
+
+    policy = MctsPolicy(env, budget=100, gamma=0.7, reuse_subtree=True)
+    a = policy.act()
+    _, _, term, trunc, _ = env.step(a)
+    policy.advance(a, term | trunc)
 """
 from __future__ import annotations
 
@@ -258,6 +266,19 @@ def opd_discount_tables(gamma: float, expansions: int):
     return g, g / (np.float64(1.0) - np.float64(gamma))
 
 
+def _check_tree_search_env(env, planner: str) -> None:
+    """The envs the tree-search planners run on: one MDPVehicle ego on an id whose `step` draws nothing from the env's
+    stream (OPD_ENV_IDS), so a row copy steps exactly like `copy.deepcopy` of the env."""
+    from .envs.common.action import DiscreteMetaAction
+
+    if getattr(env, "multi_agent", False) or getattr(env, "n_agents", 1) > 1:
+        raise NotImplementedError(f"{planner} of a multi-agent env")
+    if env.ENV_ID not in OPD_ENV_IDS:
+        raise NotImplementedError(f"{planner} on {env.ENV_ID} (supported: {', '.join(OPD_ENV_IDS)})")
+    if not isinstance(getattr(env, "action_type", None), DiscreteMetaAction):
+        raise ValueError(f"{planner} plans over the 5 DiscreteMetaAction actions of an MDPVehicle ego")
+
+
 class OpdPolicy:
     """Optimistic deterministic planning (Hren & Munos 2008; rl-agents' `DeterministicPlannerAgent`, which the
     reference's quickstart runs on highway-fast-v0 with `budget: 50, gamma: 0.7`) on the simulator itself, for every
@@ -279,14 +300,7 @@ class OpdPolicy:
     expanded) and `selected` [N, E]."""
 
     def __init__(self, env, budget: int = 50, gamma: float = 0.7):
-        from .envs.common.action import DiscreteMetaAction
-
-        if getattr(env, "multi_agent", False) or getattr(env, "n_agents", 1) > 1:
-            raise NotImplementedError("OPD of a multi-agent env")
-        if env.ENV_ID not in OPD_ENV_IDS:
-            raise NotImplementedError(f"OPD on {env.ENV_ID} (supported: {', '.join(OPD_ENV_IDS)})")
-        if not isinstance(getattr(env, "action_type", None), DiscreteMetaAction):
-            raise ValueError("OPD plans over the 5 DiscreteMetaAction actions of an MDPVehicle ego")
+        _check_tree_search_env(env, "OPD")
         if not 0.0 <= float(gamma) < 1.0:
             raise ValueError("gamma must be in [0, 1)")
         if int(budget) != budget or budget < N_ACTIONS:
@@ -358,3 +372,159 @@ class OpdPolicy:
                                            work._terminated.data_ptr(), work._truncated.data_ptr(), stream))
             N.check(lib.hwy_opd_recommend(T, stream))
         return self.actions
+
+
+MCTS_ENV_IDS = OPD_ENV_IDS
+
+
+def mcts_budget(budget: int, gamma: float):
+    """(episodes, horizon) of a budget, rl-agents' `AbstractPlanner.allocate_budget`:
+    horizon(E) = max(ceil(ln E / (2 ln(1 / gamma))), 1) and episodes = the largest E >= 1 with E * horizon(E) <= budget
+    (100 at gamma 0.7 is 20 x 5).  gamma must lie in (0, 1); a budget with no split raises ValueError."""
+    if not 0.0 < float(gamma) < 1.0:
+        raise ValueError("gamma must be in (0, 1)")
+    if int(budget) != budget or budget < 1:
+        raise ValueError(f"budget {budget} has no split into episodes x horizon (it must be an int >= 1)")
+
+    def horizon(e: int) -> int:
+        return max(int(np.ceil(np.log(np.float64(e)) / (2 * np.log(1 / np.float64(gamma))))), 1)
+
+    e = 1
+    while (e + 1) * horizon(e + 1) <= budget:
+        e += 1
+    return e, horizon(e)
+
+
+class MctsPolicy:
+    """Open-loop Monte-Carlo tree search (rl-agents' `MCTSAgent` with its `random_available` prior and rollout
+    policies) on the simulator itself, for every env of a batched env at once.  The statement it follows, with its
+    deviations from rl-agents, is tests/mcts_spec.py.
+
+    `budget` is split into `episodes` x `horizon` (`mcts_budget`).  Each episode of each root re-simulates from a copy
+    of the root's state in a *work* env of N rows (the caller's class and config, autoreset disabled): it descends the
+    tree by `value + T * n_children * prior / (count + 1)` (exact ties by a draw), expands the leaf over its available
+    actions, rolls out uniformly random available actions to the horizon, and backs the discounted return up to the
+    root.  `act()` returns int64 actions [N] on the env's device: the root child with the most visits (ties by value,
+    then the lowest action).  `temperature = 1.0` is this library's default; rl-agents' own default is not restated
+    here because it cannot be checked against the reference.
+
+    Draws come from a counter-based generator keyed by (seed, decision, root, episode, depth); `decision` counts
+    `act()` calls on the device, so a replayed CUDA graph draws fresh numbers.  A tree holds M = 1 + 5 *
+    max_expansions slots (default: `episodes`, or 4 * `episodes` with `reuse_subtree`); an expansion that does not fit
+    is skipped and counted in `tree.skipped`.
+
+    With `reuse_subtree=True`, `advance(actions, done)` after each `env.step` keeps the subtree under the action taken
+    (rl-agents' `step_strategy: "subtree"`) and clears the trees of rows that are done or whose action has no child;
+    `act()` twice without `advance()` in between raises.  Without it every `act()` starts from a bare root and
+    `advance()` does nothing.  Buffers and the work env are built at the first call (and again, with a fresh tree and
+    decision counter, only if the env's size changes); later `act()` / `advance()` calls make no host synchronisation
+    and can be captured in a CUDA graph.  The caller's env is only read.
+
+    `tree` holds [N, M] device tensors (exists, expanded, parent, action, child_base, n_children, prior, count, value),
+    `n_nodes` and `skipped` [N], and the last decision's `leaf` / `returns` [N, episodes] (the node each episode backed
+    up from and its discounted return)."""
+
+    FIELDS = ("exists", "expanded", "parent", "action", "child_base", "n_children", "prior", "count", "value")
+
+    def __init__(self, env, budget: int = 100, gamma: float = 0.7, temperature: float = 1.0, seed: int = 0,
+                 reuse_subtree: bool = False, max_expansions=None):
+        _check_tree_search_env(env, "MCTS")
+        self.episodes, self.horizon = mcts_budget(budget, gamma)
+        temperature = float(temperature)
+        if not (np.isfinite(temperature) and temperature >= 0.0):
+            raise ValueError("temperature must be finite and >= 0")
+        if max_expansions is None:
+            max_expansions = self.episodes * (4 if reuse_subtree else 1)
+        if int(max_expansions) != max_expansions or max_expansions < 1:
+            raise ValueError("max_expansions must be an int >= 1")
+        self.env, self.budget, self.gamma, self.temperature = env, int(budget), float(gamma), temperature
+        self.seed, self.reuse_subtree = int(seed) & (2**64 - 1), bool(reuse_subtree)
+        self.max_expansions = int(max_expansions)
+        self.max_nodes = 1 + N_ACTIONS * self.max_expansions
+        self._key = None
+        self._awaiting_advance = False
+        self.work = self.tree = self.actions = self.decision = None
+
+    def _allocate(self) -> None:
+        env, n, M, E, dev = self.env, self.env.num_envs, self.max_nodes, self.episodes, self.env.device
+        self.work = type(env)(config=copy.deepcopy(env.config), num_envs=n, device=dev, autoreset_mode="Disabled")
+        self.work._seeded = True  # every row is written by a row copy before anything reads it
+        z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=dev)  # noqa: E731
+        self._g = torch.from_numpy(np.float64(self.gamma) ** np.arange(self.horizon, dtype=np.float64)).to(dev)
+        self.decision = z(1, dtype=torch.int64)
+        tr = {name: z(n, M, dtype=torch.uint8) for name in ("exists", "expanded")}
+        tr.update({name: z(n, M, dtype=torch.int32) for name in ("parent", "action", "child_base", "n_children",
+                                                                 "count")})
+        tr.update({name: z(n, M, dtype=torch.float64) for name in ("prior", "value")})
+        per_root = {"n_nodes": z(n, dtype=torch.int32), "skipped": z(n, dtype=torch.int32),
+                    "walk_node": z(n, dtype=torch.int32), "walk_return": z(n, dtype=torch.float64),
+                    "walk_flags": z(n, dtype=torch.uint8), "leaf": z(n, E, dtype=torch.int32),
+                    "returns": z(n, E, dtype=torch.float64), "remap": z(n, M, dtype=torch.int32)}
+        self._work_actions = z(n, dtype=torch.int32)
+        self.actions = z(n, dtype=torch.int64)
+        self._adv_actions, self._adv_done = z(n, dtype=torch.int64), z(n, dtype=torch.uint8)
+        self._available = z(n, N_ACTIONS, dtype=torch.uint8)
+        self._buffers = {**tr, **per_root}
+        T = N.HwyMctsTree()
+        T.n_roots, T.max_nodes, T.episodes, T.horizon = n, M, E, self.horizon
+        T.temperature, T.seed = self.temperature, self.seed
+        T.discount, T.decision = self._g.data_ptr(), self.decision.data_ptr()
+        for name, buf in self._buffers.items():
+            setattr(T, name, buf.data_ptr())
+        T.actions, T.recommended = self._work_actions.data_ptr(), self.actions.data_ptr()
+        self._T = T
+        self.tree = SimpleNamespace(**{k: (v.view(torch.bool) if v.dtype == torch.uint8 else v) for k, v in tr.items()},
+                                    n_nodes=per_root["n_nodes"], skipped=per_root["skipped"], leaf=per_root["leaf"],
+                                    returns=per_root["returns"])
+        self._rows = torch.arange(n, dtype=torch.int64, device=dev)
+        self._key = (n, dev, env.V, str(env._row_layout()))
+        self._reroot(None, None)  # bare roots
+        self._awaiting_advance = False
+
+    def _reroot(self, actions, done) -> None:
+        with torch.cuda.device(self.env.device):
+            N.check(self.env._lib.hwy_mcts_reroot(C.byref(self._T), None if actions is None else actions.data_ptr(),
+                                                  None if done is None else done.data_ptr(), self.env._stream()))
+
+    def act(self) -> torch.Tensor:
+        env = self.env
+        if not env._seeded:
+            raise RuntimeError("call reset() before act()")
+        if (env.num_envs, env.device, env.V, str(env._row_layout())) != self._key:
+            self._allocate()
+        if self._awaiting_advance:
+            raise RuntimeError("reuse_subtree: call advance(actions, done) after env.step and before the next act()")
+        if not self.reuse_subtree:
+            self._reroot(None, None)
+        work, lib, T, stream = self.work, env._lib, C.byref(self._T), env._stream()
+        # the env's buffers may have been re-allocated since the last call: its table is built again
+        table = work._row_copy_table(env)
+        with torch.cuda.device(env.device):
+            for e in range(self.episodes):
+                work._copy_rows(table, self._rows, self._rows)
+                for d in range(self.horizon):
+                    work._available_actions(self._available)
+                    N.check(lib.hwy_mcts_advance(T, e, d, self._available.data_ptr(), work._reward.data_ptr(),
+                                                 work._terminated.data_ptr(), work._truncated.data_ptr(), stream))
+                    work.step(self._work_actions)
+                N.check(lib.hwy_mcts_backup(T, e, work._reward.data_ptr(), stream))
+            N.check(lib.hwy_mcts_recommend(T, stream))
+        self._awaiting_advance = self.reuse_subtree
+        return self.actions
+
+    def advance(self, actions, done) -> None:
+        """After `env.step(actions)`: re-root every tree at the child of the action taken (`reuse_subtree`), clearing
+        the rows where `done` (bool [N], e.g. terminated | truncated) or the action has no child.  A no-op without
+        `reuse_subtree`.  Device tensors keep it free of host synchronisation."""
+        if not self.reuse_subtree:
+            return
+        if self._key is None:
+            raise RuntimeError("advance() before the first act()")
+        n = self.env.num_envs
+        actions, done = torch.as_tensor(actions), torch.as_tensor(done)
+        if actions.numel() != n or done.numel() != n:
+            raise ValueError(f"advance() takes one action and one done flag per env ({n})")
+        self._adv_actions.copy_(actions.reshape(n), non_blocking=True)
+        self._adv_done.copy_(done.reshape(n), non_blocking=True)
+        self._reroot(self._adv_actions, self._adv_done)
+        self._awaiting_advance = False

@@ -666,6 +666,44 @@ int hwy_opd_record(const HwyOpdTree *t, int k, const uint8_t *available, const d
 /* recommended[r] = the root child action whose subtree holds the largest value (the lowest action on ties). */
 int hwy_opd_recommend(const HwyOpdTree *t, void *stream);
 
+/* Open-loop Monte-Carlo tree search (rl-agents' MCTSAgent; the statement is tests/mcts_spec.py) over n_roots trees of
+ * max_nodes = 1 + 5 * k slots, [n_roots][max_nodes] arrays, node 0 the root.  Expanding node p takes the 5 slots
+ * child_base[p] + a at n_nodes.  A work env of n_roots rows re-simulates each episode from the root states; the
+ * walk_* arrays carry each root's episode between the horizon's steps. */
+typedef struct HwyMctsTree {
+    int32_t n_roots, max_nodes, episodes, horizon;
+    double temperature;
+    uint64_t seed;
+    const double *discount;                  /* DEVICE [horizon]: gamma^h */
+    int64_t *decision;                       /* DEVICE [1]: act() calls so far, a key of every draw */
+    uint8_t *exists, *expanded;              /* DEVICE [n_roots][max_nodes] */
+    int32_t *parent, *action, *child_base, *n_children, *count; /* DEVICE [n_roots][max_nodes] */
+    double *prior, *value;                   /* DEVICE [n_roots][max_nodes] */
+    int32_t *n_nodes, *skipped;              /* DEVICE [n_roots]: slots in use; expansions skipped for lack of room */
+    int32_t *walk_node;                      /* DEVICE [n_roots] */
+    double *walk_return;                     /* DEVICE [n_roots] */
+    uint8_t *walk_flags;                     /* DEVICE [n_roots]: bit 0 done, bit 1 rolling out */
+    int32_t *leaf;                           /* DEVICE [n_roots][episodes]: the node each episode backed up from */
+    double *returns;                         /* DEVICE [n_roots][episodes] */
+    int32_t *remap;                          /* DEVICE [n_roots][max_nodes]: scratch of hwy_mcts_reroot */
+    int32_t *actions;                        /* DEVICE [n_roots]: the work rows' next actions */
+    int64_t *recommended;                    /* DEVICE [n_roots] */
+} HwyMctsTree;
+/* Step d of episode e: (d > 0) add the work rows' previous reward, terminated, truncated (u8 / f64 [n_roots]) to each
+ * walk, then descend, expand (over available [n_roots][5] u8) or draw a rollout action into actions; rows whose
+ * episode has ended get IDLE.  d == 0 starts the walk at the root; (e, d) == (0, 0) also zeroes skipped. */
+int hwy_mcts_advance(const HwyMctsTree *t, int e, int d, const uint8_t *available, const double *reward,
+                     const uint8_t *terminated, const uint8_t *truncated, void *stream);
+/* End of episode e: add the last step's reward (f64 [n_roots]) to each walk that has not ended, back the return up
+ * from the walk's node to the root and record leaf / returns [., e]. */
+int hwy_mcts_backup(const HwyMctsTree *t, int e, const double *reward, void *stream);
+/* recommended[r] = the root child with the largest count, ties by value then lowest action; decision += 1. */
+int hwy_mcts_recommend(const HwyMctsTree *t, void *stream);
+/* Subtree reuse: root r's child for actions[r] (int64) becomes the root, its subtree compacted to the front in index
+ * order; roots with done[r] (u8) or without that child are cleared to a bare root.  actions = done = NULL clears every
+ * tree. */
+int hwy_mcts_reroot(const HwyMctsTree *t, const int64_t *actions, const uint8_t *done, void *stream);
+
 /* Kernel launches issued by the calling thread through this library since load (the
  * `gpu_launches` claim of bench.py). */
 uint64_t hwy_launch_count(void);
