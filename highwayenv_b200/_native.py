@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HWYB200_LIB") or os.path.join(_HERE, "csrc", "libhwyb200.so")
 
-HWY_ABI_VERSION = 15 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
+HWY_ABI_VERSION = 16 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
 HWY_MAX_LANES = 8
 HWY_MAX_TARGET_SPEEDS = 8
 HWY_MAX_VEHICLES = 128
@@ -282,13 +282,12 @@ class HwyLidarParams(C.Structure):
 EXPORTS = (
     "hwy_observe_grid", "hwy_observe_ttc", "hwy_observe_lidar", "hwy_exit_reset",
     "hwy_abi_version", "hwy_last_error", "hwy_highway_slot_stride", "hwy_highway_reset",
-    "hwy_highway_observe", "hwy_highway_step", "hwy_highway_autoreset", "hwy_highway_substeps", "hwy_launch_count",
+    "hwy_highway_observe", "hwy_highway_step", "hwy_highway_substeps", "hwy_launch_count",
     "hwy_network_obs_size", "hwy_network_step", "hwy_network_observe", "hwy_roundabout_reset",
-    "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset", "hwy_intersection_step_agents",
+    "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset",
     "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
-    "hwy_value_iteration", "hwy_highway_linear_reset", "hwy_highway_linear_step", "hwy_highway_linear_autoreset",
-    "hwy_highway_linear_substeps", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
+    "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
 )
 
@@ -319,28 +318,18 @@ def load():
     lib.hwy_launch_count.restype = C.c_uint64
     lib.hwy_highway_slot_stride.restype = C.c_int
     lib.hwy_highway_slot_stride.argtypes = [C.c_int]
-    P, S = C.POINTER(HwyHighwayParams), C.POINTER(HwyHighwayState)
+    # the highway reset / step / substeps take the LinearVehicle traffic T (None: IDMVehicle traffic)
+    P, S, T = C.POINTER(HwyHighwayParams), C.POINTER(HwyHighwayState), C.POINTER(HwyLinearTraffic)
     lib.hwy_highway_reset.restype = C.c_int
-    lib.hwy_highway_reset.argtypes = [P, S, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_highway_reset.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_highway_observe.restype = C.c_int
     lib.hwy_highway_observe.argtypes = [P, S, C.c_void_p, C.c_void_p]
     lib.hwy_highway_step.restype = C.c_int
-    lib.hwy_highway_step.argtypes = [P, S, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+    lib.hwy_highway_step.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                      C.c_void_p, C.c_void_p]
     lib.hwy_highway_substeps.restype = C.c_int
-    lib.hwy_highway_substeps.argtypes = [P, S, C.c_int, C.c_void_p, C.c_void_p]
-    lib.hwy_highway_autoreset.restype = C.c_int
-    lib.hwy_highway_autoreset.argtypes = [P, S, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    T = C.POINTER(HwyLinearTraffic)
-    lib.hwy_highway_linear_reset.restype = C.c_int
-    lib.hwy_highway_linear_reset.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.hwy_highway_linear_step.restype = C.c_int
-    lib.hwy_highway_linear_step.argtypes = [P, S, T] + lib.hwy_highway_step.argtypes[2:]
-    lib.hwy_highway_linear_substeps.restype = C.c_int
-    lib.hwy_highway_linear_substeps.argtypes = [P, S, T, C.c_int, C.c_void_p, C.c_void_p]
-    lib.hwy_highway_linear_autoreset.restype = C.c_int
-    lib.hwy_highway_linear_autoreset.argtypes = [P, S, T, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_highway_substeps.argtypes = [P, S, T, C.c_int, C.c_void_p, C.c_void_p]
     NP, NG, NS = C.POINTER(HwyNetParams), C.c_void_p, C.POINTER(HwyNetState)
     lib.hwy_network_obs_size.restype = C.c_int
     lib.hwy_network_obs_size.argtypes = [NP]
@@ -350,10 +339,7 @@ def load():
     lib.hwy_network_observe.restype = C.c_int
     lib.hwy_network_observe.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p]
     lib.hwy_intersection_step.restype = C.c_int
-    lib.hwy_intersection_step.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.hwy_intersection_step_agents.restype = C.c_int
-    lib.hwy_intersection_step_agents.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS] + [C.c_void_p] * 10
+    lib.hwy_intersection_step.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS] + [C.c_void_p] * 10
     lib.hwy_debug_network_neighbours.restype = C.c_int
     lib.hwy_debug_network_neighbours.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_debug_rotated_rectangles_intersect.restype = C.c_int

@@ -1576,35 +1576,54 @@ int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const ui
     return check_launch("highway_observe_kernel");
 }
 
-int launch_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask_a,
-                 const uint8_t* mask_b, cudaStream_t st) {
+// t == nullptr: IDMVehicle traffic (highway_reset_kernel); else LinearVehicle traffic (highway_linear_reset_kernel)
+int launch_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                 const uint8_t* mask_a, const uint8_t* mask_b, cudaStream_t st) {
     int blocks = (s->n_envs + 127) / 128;
+    if (t) {
+        hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b);
+        return check_launch("highway_linear_reset_kernel");
+    }
     hwy::highway_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, mask_a, mask_b);
     return check_launch("highway_reset_kernel");
 }
 
-int launch_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                        const uint8_t* mask_a, const uint8_t* mask_b, cudaStream_t st) {
-    int blocks = (s->n_envs + 127) / 128;
-    hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b);
-    return check_launch("highway_linear_reset_kernel");
-}
-
-int validate_linear(const HwyLinearTraffic* t) {
-    if (!t || !t->params) return fail("%s", "null linear traffic parameters");
+int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                    const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                    int autoreset) {
+    if (validate(p, s)) return 1;
+    if (!obs || !reward || !terminated || !truncated) return fail("%s", "null output pointer");
+    if (p->action_type == 0 && !action_i) return fail("%s", "DiscreteMetaAction needs action_i");
+    if (p->action_type == 1 && !action_f) return fail("%s", "ContinuousAction needs action_f");
+    if (autoreset != HWY_AUTORESET_DISABLED && autoreset != HWY_AUTORESET_SAME_STEP)
+        return fail("%s", "unknown autoreset mode");
     return 0;
 }
-}  // namespace
 
-namespace {
 int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
                   const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
                   uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
-                  cudaStream_t st);
-int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                    const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
-                    int autoreset);
+                  cudaStream_t st) {
+    int tpe = tpe_for(p->n_vehicles);
+    // HWYB200_GENERAL_LANES=1 (tests): run the general-geometry instantiation on a congruent lane table too
+    const char* force_general = getenv("HWYB200_GENERAL_LANES");
+    const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
+#define HWY_LAUNCH_STEP(T, A)                                                                              \
+    launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
+                      autoreset, final_obs, st)
+    int rc;
+    if (tpe == 32)
+        rc = al ? HWY_LAUNCH_STEP(32, true) : HWY_LAUNCH_STEP(32, false);
+    else if (tpe == 64)
+        rc = al ? HWY_LAUNCH_STEP(64, true) : HWY_LAUNCH_STEP(64, false);
+    else
+        rc = al ? HWY_LAUNCH_STEP(128, true) : HWY_LAUNCH_STEP(128, false);
+#undef HWY_LAUNCH_STEP
+    if (rc) return 1;
+    if (check_launch(t ? "highway_linear_step_kernel" : "highway_step_kernel")) return 1;
+    return 0;
 }
+}  // namespace
 
 extern "C" {
 
@@ -1619,13 +1638,14 @@ int hwy_highway_observe(const HwyHighwayParams* p, const HwyHighwayState* s, flo
     return launch_observe(p, s, nullptr, nullptr, obs, (cudaStream_t)stream);
 }
 
-int hwy_highway_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask,
-                      float* obs, void* stream) {
+int hwy_highway_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                      const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
+    if (t && !t->params) return fail("%s", "null linear traffic parameters");
     if (validate(p, s)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     if (ensure_pcg_jump(st)) return 1;  // the fused autoreset of later steps reads the table
-    if (launch_reset(p, s, mask, nullptr, st)) return 1;
-    if (obs) return launch_observe(p, s, mask, nullptr, obs, st);
+    if (launch_reset(p, s, t, mask_a, mask_b, st)) return 1;
+    if (obs) return launch_observe(p, s, mask_a, mask_b, obs, st);
     return 0;
 }
 
@@ -1669,108 +1689,24 @@ int hwy_debug_pcg64(int op, int arg_i, double arg_lo, double arg_hi, int count, 
     return check_launch("debug_pcg64_kernel");
 }
 
-int hwy_highway_autoreset(const HwyHighwayParams* p, const HwyHighwayState* s,
-                          const uint8_t* terminated, const uint8_t* truncated, float* obs,
-                          void* stream) {
-    if (validate(p, s)) return 1;
-    if (!terminated || !truncated || !obs) return fail("%s", "null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (launch_reset(p, s, terminated, truncated, st)) return 1;
-    return launch_observe(p, s, terminated, truncated, obs, st);
-}
-
-int hwy_highway_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                     const float* action_f, float* obs, double* reward, uint8_t* terminated,
-                     uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset,
-                     float* final_obs, void* stream) {
+int hwy_highway_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                     const int32_t* action_i, const float* action_f, float* obs, double* reward,
+                     uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
+                     int autoreset, float* final_obs, void* stream) {
+    if (t && !t->params) return fail("%s", "null linear traffic parameters");
     if (check_step_args(p, s, action_i, action_f, obs, reward, terminated, truncated, autoreset)) return 1;
-    return dispatch_step(p, s, nullptr, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-                         autoreset, final_obs, (cudaStream_t)stream);
-}
-
-/* B4 seam of the reference (abstract.py:304-307 minus action_type.act): n_substeps x (Road.act(); Road.step(dt)). */
-int hwy_highway_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, int n_substeps, const float* action_f,
-                         void* stream) {
-    if (validate(p, s)) return 1;
-    if (n_substeps < 1 || n_substeps > 4096) return fail("%s", "n_substeps must be in 1..4096");
-    return dispatch_step(p, s, nullptr, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                         -n_substeps, nullptr, (cudaStream_t)stream);
-}
-
-// ---- LinearVehicle traffic: the same four entry points on the linear kernels
-int hwy_highway_linear_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                             const uint8_t* mask, float* obs, void* stream) {
-    if (validate(p, s) || validate_linear(t)) return 1;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (ensure_pcg_jump(st)) return 1;
-    if (launch_linear_reset(p, s, t, mask, nullptr, st)) return 1;
-    if (obs) return launch_observe(p, s, mask, nullptr, obs, st);
-    return 0;
-}
-
-int hwy_highway_linear_autoreset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                                 const uint8_t* terminated, const uint8_t* truncated, float* obs, void* stream) {
-    if (validate(p, s) || validate_linear(t)) return 1;
-    if (!terminated || !truncated || !obs) return fail("%s", "null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (launch_linear_reset(p, s, t, terminated, truncated, st)) return 1;
-    return launch_observe(p, s, terminated, truncated, obs, st);
-}
-
-int hwy_highway_linear_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                            const int32_t* action_i, const float* action_f, float* obs, double* reward,
-                            uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                            int autoreset, float* final_obs, void* stream) {
-    if (check_step_args(p, s, action_i, action_f, obs, reward, terminated, truncated, autoreset)) return 1;
-    if (validate_linear(t)) return 1;
     return dispatch_step(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
                          autoreset, final_obs, (cudaStream_t)stream);
 }
 
-int hwy_highway_linear_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                                int n_substeps, const float* action_f, void* stream) {
-    if (validate(p, s) || validate_linear(t)) return 1;
+/* B4 seam of the reference (abstract.py:304-307 minus action_type.act): n_substeps x (Road.act(); Road.step(dt)). */
+int hwy_highway_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
+                         int n_substeps, const float* action_f, void* stream) {
+    if (t && !t->params) return fail("%s", "null linear traffic parameters");
+    if (validate(p, s)) return 1;
     if (n_substeps < 1 || n_substeps > 4096) return fail("%s", "n_substeps must be in 1..4096");
     return dispatch_step(p, s, t, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                          -n_substeps, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"
-
-namespace {
-int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                    const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
-                    int autoreset) {
-    if (validate(p, s)) return 1;
-    if (!obs || !reward || !terminated || !truncated) return fail("%s", "null output pointer");
-    if (p->action_type == 0 && !action_i) return fail("%s", "DiscreteMetaAction needs action_i");
-    if (p->action_type == 1 && !action_f) return fail("%s", "ContinuousAction needs action_f");
-    if (autoreset != HWY_AUTORESET_DISABLED && autoreset != HWY_AUTORESET_SAME_STEP)
-        return fail("%s", "unknown autoreset mode");
-    return 0;
-}
-
-int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                  const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
-                  uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
-                  cudaStream_t st) {
-    int tpe = tpe_for(p->n_vehicles);
-    // HWYB200_GENERAL_LANES=1 (tests): run the general-geometry instantiation on a congruent lane table too
-    const char* force_general = getenv("HWYB200_GENERAL_LANES");
-    const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
-#define HWY_LAUNCH_STEP(T, A)                                                                              \
-    launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
-                      autoreset, final_obs, st)
-    int rc;
-    if (tpe == 32)
-        rc = al ? HWY_LAUNCH_STEP(32, true) : HWY_LAUNCH_STEP(32, false);
-    else if (tpe == 64)
-        rc = al ? HWY_LAUNCH_STEP(64, true) : HWY_LAUNCH_STEP(64, false);
-    else
-        rc = al ? HWY_LAUNCH_STEP(128, true) : HWY_LAUNCH_STEP(128, false);
-#undef HWY_LAUNCH_STEP
-    if (rc) return 1;
-    if (check_launch(t ? "highway_linear_step_kernel" : "highway_step_kernel")) return 1;
-    return 0;
-}
-}  // namespace

@@ -2531,15 +2531,7 @@ int hwy_network_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyN
 int hwy_intersection_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
                           const HwyNetState* s, const int32_t* action, float* obs, double* reward,
                           uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                          void* stream) {
-    return hwy_intersection_step_agents(p, graph, spawn, s, action, obs, reward, terminated, truncated, info_speed,
-                                        info_crashed, nullptr, nullptr, stream);
-}
-
-int hwy_intersection_step_agents(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
-                                 const HwyNetState* s, const int32_t* action, float* obs, double* reward,
-                                 uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                                 double* agents_reward, uint8_t* agents_terminated, void* stream) {
+                          double* agents_reward, uint8_t* agents_terminated, void* stream) {
     if (validate_net(p, graph, s)) return 1;
     if (p->n_agents > 1 && (p->obs_type != HWY_OBS_KINEMATICS || p->reward_type != 1))
         return fail("%s", "several controlled vehicles: Kinematics observation on intersection envs only");

@@ -202,6 +202,8 @@ class BatchedHighwayEnv(BatchedVectorEnv):
             t.acc_lo[:], t.acc_span[:] = [float(x) for x in acc_lo], [float(x) for x in acc_span]
             t.steer_lo[:], t.steer_span[:] = [float(x) for x in steer_lo], [float(x) for x in steer_span]
             self._traffic = t
+        # the traffic argument of the reset / step / substeps entry points (None: IDMVehicle traffic)
+        self._traffic_arg = None if self._traffic is None else C.byref(self._traffic)
         self._allocated_for = key
 
     # ------------------------------------------------------------------ family kernels
@@ -212,18 +214,9 @@ class BatchedHighwayEnv(BatchedVectorEnv):
 
     def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
         """Re-spawn the envs set in mask_a or mask_b (every env without masks) from their streams."""
-        lib, P, S = self._lib, C.byref(self._params), C.byref(self._state)
         with torch.cuda.device(self.device):
-            if self._traffic is not None:
-                T = C.byref(self._traffic)
-                if mask_b is None:
-                    N.check(lib.hwy_highway_linear_reset(P, S, T, mask_a, obs_ptr, self._stream()))
-                else:
-                    N.check(lib.hwy_highway_linear_autoreset(P, S, T, mask_a, mask_b, obs_ptr, self._stream()))
-            elif mask_b is None:
-                N.check(lib.hwy_highway_reset(P, S, mask_a, obs_ptr, self._stream()))
-            else:
-                N.check(lib.hwy_highway_autoreset(P, S, mask_a, mask_b, obs_ptr, self._stream()))
+            N.check(self._lib.hwy_highway_reset(C.byref(self._params), C.byref(self._state), self._traffic_arg,
+                                                mask_a, mask_b, obs_ptr, self._stream()))
 
     def _step_kernels(self, act) -> None:
         ai = act.data_ptr() if self._params.action_type == 0 else None
@@ -235,11 +228,7 @@ class BatchedHighwayEnv(BatchedVectorEnv):
                 N.AUTORESET_SAME_STEP if fused_reset else N.AUTORESET_DISABLED,
                 self._final_obs.data_ptr() if fused_reset else None, self._stream())
         with torch.cuda.device(self.device):
-            if self._traffic is not None:
-                N.check(self._lib.hwy_highway_linear_step(C.byref(self._params), C.byref(self._state),
-                                                          C.byref(self._traffic), *args))
-            else:
-                N.check(self._lib.hwy_highway_step(C.byref(self._params), C.byref(self._state), *args))
+            N.check(self._lib.hwy_highway_step(C.byref(self._params), C.byref(self._state), self._traffic_arg, *args))
 
     def _same_step_autoreset(self, info) -> None:
         if self._plugin_standalone:
@@ -301,13 +290,8 @@ class BatchedHighwayEnv(BatchedVectorEnv):
                 raise ValueError("pass the continuous (throttle, steering) pair, not a DiscreteAction index")
             af = self._stage_actions(action).data_ptr()
         with torch.cuda.device(self.device):
-            if self._traffic is not None:
-                N.check(self._lib.hwy_highway_linear_substeps(C.byref(self._params), C.byref(self._state),
-                                                              C.byref(self._traffic), int(n_substeps), af,
-                                                              self._stream()))
-            else:
-                N.check(self._lib.hwy_highway_substeps(C.byref(self._params), C.byref(self._state), int(n_substeps),
-                                                       af, self._stream()))
+            N.check(self._lib.hwy_highway_substeps(C.byref(self._params), C.byref(self._state), self._traffic_arg,
+                                                   int(n_substeps), af, self._stream()))
 
     def _env_rows(self) -> dict:
         rows = super()._env_rows()

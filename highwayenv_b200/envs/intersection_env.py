@@ -331,7 +331,7 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
 
     def _step_kernels(self, act) -> None:
         with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_intersection_step_agents(
+            N.check(self._lib.hwy_intersection_step(
                 C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
                 act.data_ptr(), self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
                 self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),

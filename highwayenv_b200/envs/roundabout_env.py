@@ -244,7 +244,7 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
                     C.byref(self._params), self._graph_dev.data_ptr(), None, C.byref(self._state), act.data_ptr(),
                     self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
                     self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
-                    self._stream()))
+                    None, None, self._stream()))
 
     def get_available_actions(self) -> torch.Tensor:
         """DiscreteMetaAction.get_available_actions (envs/common/action.py:262-298, AbstractEnv.get_available_actions

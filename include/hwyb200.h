@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define HWY_ABI_VERSION 15
+#define HWY_ABI_VERSION 16
 #define HWY_MAX_LANES 8
 #define HWY_MAX_TARGET_SPEEDS 8
 #define HWY_MAX_VEHICLES 128 /* per env, incl. the ego */
@@ -150,13 +150,33 @@ const char *hwy_last_error(void);
 /* Slot stride for n_vehicles (next multiple of 2; 128-bit alignment of the packed pairs). */
 int hwy_highway_slot_stride(int n_vehicles);
 
-/* AbstractEnv.reset()'s _reset() for the envs whose mask byte is non-zero (mask == NULL:
- * all): HighwayEnv._create_road/_create_vehicles (highway_env.py:55-98,177-182) with
+/* LinearVehicle traffic (vehicle/behavior.py:350-583; AggressiveVehicle and DefensiveVehicle
+ * are the same model on the highway, they differ only in p->lane_change_min_acc_gain).  Every
+ * traffic vehicle keeps the parameters randomize_behavior drew for it (behavior.py:406-415):
+ *   params[5*(e*vp+v) + 0..2] = ACCELERATION_PARAMETERS, + 3..4 = STEERING_PARAMETERS
+ * (DEVICE, [n_envs*vp*5] doubles; the controlled vehicle's row is zero).  A reset draws
+ *   ACCELERATION_PARAMETERS = acc_lo + uniform(size=3) * acc_span,
+ *   STEERING_PARAMETERS     = steer_lo + uniform(size=2) * steer_span
+ * with acc_lo = ACCELERATION_RANGE[0], acc_span = ACCELERATION_RANGE[1] - ACCELERATION_RANGE[0]
+ * (likewise steering) as numpy evaluates them on the host.  p->time_wanted is the class's
+ * TIME_WANTED (2.5).  The reset, step and substeps entry points below take a `t` argument:
+ * NULL runs IDMVehicle traffic, non-NULL (with t->params set) runs this traffic model. */
+#define HWY_LINEAR_PARAMS 5
+typedef struct HwyLinearTraffic {
+    double *params;
+    double acc_lo[3], acc_span[3];
+    double steer_lo[2], steer_span[2];
+} HwyLinearTraffic;
+
+/* AbstractEnv.reset()'s _reset() for the envs with mask_a[e] | mask_b[e] (both NULL: every
+ * env): HighwayEnv._create_road/_create_vehicles (highway_env.py:55-98,177-182) with
  * Vehicle.create_random (kinematics.py:50-104), drawing from each env's PCG64 stream in
  * the reference's order.  If obs != NULL also writes the reset observation
- * [n_envs][obs_vehicles_count][n columns] float32 of those envs. */
-int hwy_highway_reset(const HwyHighwayParams *p, const HwyHighwayState *s, const uint8_t *mask,
-                      float *obs, void *stream);
+ * [n_envs][obs_vehicles_count][n columns] float32 of those envs.  With mask_a = terminated
+ * and mask_b = truncated this is the SameStep autoreset half of hwy_highway_step on its own
+ * (lets a caller time / schedule the two halves separately). */
+int hwy_highway_reset(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                      const uint8_t *mask_a, const uint8_t *mask_b, float *obs, void *stream);
 
 /* KinematicObservation.observe() (observation.py:234-276) for all envs. */
 int hwy_highway_observe(const HwyHighwayParams *p, const HwyHighwayState *s, float *obs,
@@ -174,10 +194,10 @@ int hwy_highway_observe(const HwyHighwayParams *p, const HwyHighwayState *s, flo
  *   autoreset = HWY_AUTORESET_SAME_STEP: envs that ended are reset from their RNG stream
  *   in the same call and `obs` holds the reset observation; `final_obs` (may be NULL)
  *   receives the pre-reset observation of every env. */
-int hwy_highway_step(const HwyHighwayParams *p, const HwyHighwayState *s, const int32_t *action_i,
-                     const float *action_f, float *obs, double *reward, uint8_t *terminated,
-                     uint8_t *truncated, double *info_speed, uint8_t *info_crashed, int autoreset,
-                     float *final_obs, void *stream);
+int hwy_highway_step(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                     const int32_t *action_i, const float *action_f, float *obs, double *reward,
+                     uint8_t *terminated, uint8_t *truncated, double *info_speed, uint8_t *info_crashed,
+                     int autoreset, float *final_obs, void *stream);
 
 /* The operator seam `_simulate` uses (envs/common/abstract.py:304-307 without action_type.act):
  * `n_substeps` times  Road.act()  (road/road.py:464-467)  then  Road.step(1 / simulation_frequency)  (:469-481)
@@ -185,44 +205,8 @@ int hwy_highway_step(const HwyHighwayParams *p, const HwyHighwayState *s, const 
  * ControlledVehicle.act(None) (its current target lane / speed); a ContinuousAction ego keeps the action dict given in
  * `action_f` ([n_envs, 2] in [-1, 1], as for hwy_highway_step) or the default {steering 0, acceleration 0} if NULL.
  * What BASELINE.md's "Road.act() + Road.step(dt)" timing runs. */
-int hwy_highway_substeps(const HwyHighwayParams *p, const HwyHighwayState *s, int n_substeps, const float *action_f,
-                         void *stream);
-
-/* The SameStep autoreset half of hwy_highway_step on its own: re-spawn the envs whose
- * terminated | truncated byte is set and overwrite their rows of `obs` with the reset
- * observation (lets a caller time / schedule the two halves separately). */
-int hwy_highway_autoreset(const HwyHighwayParams *p, const HwyHighwayState *s,
-                          const uint8_t *terminated, const uint8_t *truncated, float *obs,
-                          void *stream);
-
-/* LinearVehicle traffic (vehicle/behavior.py:350-583; AggressiveVehicle and DefensiveVehicle
- * are the same model on the highway, they differ only in p->lane_change_min_acc_gain).  Every
- * traffic vehicle keeps the parameters randomize_behavior drew for it (behavior.py:406-415):
- *   params[5*(e*vp+v) + 0..2] = ACCELERATION_PARAMETERS, + 3..4 = STEERING_PARAMETERS
- * (DEVICE, [n_envs*vp*5] doubles; the controlled vehicle's row is zero).  A reset draws
- *   ACCELERATION_PARAMETERS = acc_lo + uniform(size=3) * acc_span,
- *   STEERING_PARAMETERS     = steer_lo + uniform(size=2) * steer_span
- * with acc_lo = ACCELERATION_RANGE[0], acc_span = ACCELERATION_RANGE[1] - ACCELERATION_RANGE[0]
- * (likewise steering) as numpy evaluates them on the host.  p->time_wanted is the class's
- * TIME_WANTED (2.5).  The _linear entry points are the IDM ones with this traffic model. */
-#define HWY_LINEAR_PARAMS 5
-typedef struct HwyLinearTraffic {
-    double *params;
-    double acc_lo[3], acc_span[3];
-    double steer_lo[2], steer_span[2];
-} HwyLinearTraffic;
-
-int hwy_highway_linear_reset(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
-                             const uint8_t *mask, float *obs, void *stream);
-int hwy_highway_linear_step(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
-                            const int32_t *action_i, const float *action_f, float *obs, double *reward,
-                            uint8_t *terminated, uint8_t *truncated, double *info_speed, uint8_t *info_crashed,
-                            int autoreset, float *final_obs, void *stream);
-int hwy_highway_linear_substeps(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
-                                int n_substeps, const float *action_f, void *stream);
-int hwy_highway_linear_autoreset(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
-                                 const uint8_t *terminated, const uint8_t *truncated, float *obs, void *stream);
-
+int hwy_highway_substeps(const HwyHighwayParams *p, const HwyHighwayState *s, const HwyLinearTraffic *t,
+                         int n_substeps, const float *action_f, void *stream);
 
 /* ====================================================================== general road networks
  * roundabout-v0 (envs/roundabout_env.py): Straight / Sine / Circular lanes (road/lane.py:159-384),
@@ -374,22 +358,17 @@ int hwy_network_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyN
 
 /* Same for intersection-v0 (s->vp == HWY_NET_GROUP_LARGE): RegulatedRoad rules every
  * int(simulation_frequency / 2) substeps, and after the observation the step's _clear_vehicles and
- * _spawn_vehicle(spawn_probability) drawing from s->rng (IntersectionEnv.step, :136-140). */
+ * _spawn_vehicle(spawn_probability) drawing from s->rng (IntersectionEnv.step, :136-140).
+ * With config["controlled_vehicles"] = p->n_agents > 1 (intersection-multi-agent-v0,
+ * envs/intersection_env.py:376-420): action [n_envs][n_agents], obs [n_envs][n_agents][K][F]; reward is the mean
+ * of the agents' rewards, terminated = any crashed or all arrived (:62-134); agents_reward / agents_terminated
+ * [n_envs][n_agents] (NULL for a single agent; optional) are _info's per-agent entries, which MultiAgentWrapper
+ * (abstract.py:468-477) returns in place of the scalar reward / terminated. */
 int hwy_intersection_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyIntersectionSpawn *spawn,
                           const HwyNetState *s, const int32_t *action, float *obs, double *reward,
                           uint8_t *terminated, uint8_t *truncated, double *info_speed,
-                          uint8_t *info_crashed, void *stream);
-
-/* The same with config["controlled_vehicles"] = p->n_agents > 1 (intersection-multi-agent-v0,
- * envs/intersection_env.py:376-420): action [n_envs][n_agents], obs [n_envs][n_agents][K][F]; reward is the mean
- * of the agents' rewards, terminated = any crashed or all arrived (:62-134); agents_reward / agents_terminated
- * [n_envs][n_agents] (optional) are _info's per-agent entries, which MultiAgentWrapper (abstract.py:468-477)
- * returns in place of the scalar reward / terminated. */
-int hwy_intersection_step_agents(const HwyNetParams *p, const HwyNetGraph *graph, const HwyIntersectionSpawn *spawn,
-                                 const HwyNetState *s, const int32_t *action, float *obs, double *reward,
-                                 uint8_t *terminated, uint8_t *truncated, double *info_speed,
-                                 uint8_t *info_crashed, double *agents_reward, uint8_t *agents_terminated,
-                                 void *stream);
+                          uint8_t *info_crashed, double *agents_reward, uint8_t *agents_terminated,
+                          void *stream);
 
 /* IntersectionEnv._reset / _make_vehicles (envs/intersection_env.py:119-122,245-323) on the device for the
  * envs with mask_a[e] | mask_b[e] (both NULL: every env): n-1 _spawn_vehicle draws, 3 s of warm-up simulation,

@@ -235,7 +235,7 @@ def test_abi_errors_are_loud():
     from highwayenv_b200 import _native as N
 
     lib = N.load()
-    assert lib.hwy_highway_step(None, None, None, None, None, None, None, None, None, None, 0, None, None) != 0
+    assert lib.hwy_highway_step(None, None, None, None, None, None, None, None, None, None, None, 0, None, None) != 0
     assert b"null" in lib.hwy_last_error()
     import highwayenv_b200 as hb
 

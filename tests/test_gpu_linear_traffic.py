@@ -133,9 +133,9 @@ def test_teacher_forced_vs_oracle_many_envs(name, n, T):
 @pytest.mark.parametrize("name,n", [("linear_highway_fast_v20", 128), ("linear_aggressive_fast_v50", 64),
                                     ("linear_highway_v100_continuous", 16)])
 def test_fused_autoreset_equals_linear_reset(name, n):
-    """Envs re-spawned by the SameStep autoreset inside the step kernel equal hwy_highway_linear_reset (the oracle's
-    reset): state, parameters and generator words — on 32, 64 and 128 threads per env (V = 101 jumps past the
-    PCG64 table in several hops)."""
+    """Envs re-spawned by the SameStep autoreset inside the step kernel equal hwy_highway_reset with LinearVehicle
+    traffic (the oracle's reset): state, parameters and generator words — on 32, 64 and 128 threads per env
+    (V = 101 jumps past the PCG64 table in several hops)."""
     cfg = dict(load_golden(name)["config"])
     cfg["duration"] = 2  # frequent truncation
     oc, ob = _oracle(cfg, n, 11000)
@@ -258,7 +258,8 @@ def test_state_dict_round_trip_and_idm_dicts_unchanged():
 
 
 def test_road_substeps_and_single_env():
-    """hwy_highway_linear_substeps against the oracle's orc_linear_highway_substeps; make_single on linear traffic."""
+    """hwy_highway_substeps with LinearVehicle traffic against the oracle's orc_linear_highway_substeps; make_single
+    on linear traffic."""
     import highwayenv_b200 as hb
 
     g = load_golden("linear_highway_fast_v20")

@@ -18,7 +18,7 @@ def test_library_exports_every_declared_symbol():
     lib = N.load()
     hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
     declared = set(re.findall(r"\b(hwy_[a-z_0-9]+)\s*\(", hdr))
-    assert {"hwy_highway_step", "hwy_highway_reset", "hwy_highway_observe", "hwy_highway_autoreset",
+    assert {"hwy_highway_step", "hwy_highway_reset", "hwy_highway_observe", "hwy_highway_substeps",
             "hwy_highway_slot_stride", "hwy_abi_version", "hwy_last_error", "hwy_launch_count",
             "hwy_debug_math", "hwy_debug_pcg64"} <= declared
     assert declared <= set(N.EXPORTS) | {"hwy_debug_phase_cycles"}
@@ -57,7 +57,7 @@ def test_abi_validation_without_gpu():
     from highwayenv_b200 import _native as N
 
     lib = N.load()
-    assert lib.hwy_highway_step(None, None, None, None, None, None, None, None, None, None, 0, None, None) != 0
+    assert lib.hwy_highway_step(None, None, None, None, None, None, None, None, None, None, None, 0, None, None) != 0
     assert b"null" in lib.hwy_last_error()
     p, s = N.HwyHighwayParams(), N.HwyHighwayState()
     p.n_vehicles = 500

@@ -134,10 +134,19 @@ def test_linear_entries_and_struct():
     from highwayenv_b200 import _native as N
 
     lib = N.load()
+    # LinearVehicle traffic is the `t` argument of the unified entries, not a second set of entry points
+    hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
     for sym in ("hwy_highway_linear_reset", "hwy_highway_linear_step", "hwy_highway_linear_autoreset",
-                "hwy_highway_linear_substeps"):
-        assert sym in N.EXPORTS and getattr(lib, sym) is not None
-    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 15
+                "hwy_highway_linear_substeps", "hwy_highway_autoreset"):
+        assert sym not in N.EXPORTS and sym not in hdr, sym
+    # a traffic struct without its parameter buffer is refused before any device call
+    p, s, t = N.HwyHighwayParams(), N.HwyHighwayState(), N.HwyLinearTraffic()
+    P, S, T = C.byref(p), C.byref(s), C.byref(t)
+    for rc in (lib.hwy_highway_reset(P, S, T, None, None, None, None),
+               lib.hwy_highway_step(P, S, T, None, None, None, None, None, None, None, None, 0, None, None),
+               lib.hwy_highway_substeps(P, S, T, 1, None, None)):
+        assert rc != 0 and b"null linear traffic parameters" in lib.hwy_last_error()
+    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 16
     src = ('#include <stdio.h>\n#include <stddef.h>\n#include "hwyb200.h"\nint main(){printf("%zu %zu %zu %zu %zu %d\\n", '
            'sizeof(HwyLinearTraffic), offsetof(HwyLinearTraffic, acc_span), offsetof(HwyLinearTraffic, steer_lo), '
            'offsetof(HwyLinearTraffic, steer_span), offsetof(HwyLinearTraffic, acc_lo), HWY_LINEAR_PARAMS);return 0;}\n')
