@@ -40,6 +40,8 @@ REGISTRY = {
     "intersection-multi-agent-v0": "highwayenv_b200.envs.intersection_env:BatchedMultiAgentIntersectionEnv",
     "intersection-multi-agent-v1": "highwayenv_b200.envs.intersection_env:BatchedMultiAgentWrappedIntersectionEnv",
     "intersection-multi-agent-v2": "highwayenv_b200.envs.intersection_env:BatchedConnectedLaneMultiAgentIntersectionEnv",
+    # one dynamical BicycleVehicle on a sine lane, Dict observation, TimeLimit(max_episode_steps=200)
+    "lane-keeping-v0": "highwayenv_b200.envs.lane_keeping_env:BatchedLaneKeepingEnv",
 }
 
 

@@ -279,6 +279,24 @@ class HwyLidarParams(C.Structure):
     _fields_ = [("cells", C.c_int32), ("normalize", C.c_int32), ("maximum_range", C.c_double)]
 
 
+# ---- lane-keeping-v0
+HWY_LK_MAX_ATTR = 3
+LK_ATTRIBUTES = {"state": 0, "derivative": 1, "reference_state": 2}  # HwyLaneKeepingParams.attr codes
+
+
+class HwyLaneKeepingParams(C.Structure):
+    _fields_ = ([("frames", C.c_int32), ("n_attr", C.c_int32), ("attr", C.c_int32 * HWY_LK_MAX_ATTR)]
+                + [(n, C.c_int32) for n in ("longitudinal", "lateral", "act_clip", "max_episode_steps", "autoreset")]
+                + [(n, C.c_double) for n in ("dt", "state_noise", "derivative_noise", "acc_lo", "acc_hi", "steer_lo",
+                                             "steer_hi", "x0", "y0", "heading0", "speed0")]
+                + [("lanes", HwyNetLane * 2)])
+
+
+class HwyLaneKeepingState(C.Structure):
+    _fields_ = [("n_envs", C.c_int32), ("_pad", C.c_int32), ("state", C.c_void_p), ("lane_phase", C.c_void_p),
+                ("elapsed", C.c_void_p), ("rng", C.c_void_p)]
+
+
 EXPORTS = (
     "hwy_observe_grid", "hwy_observe_ttc", "hwy_observe_lidar", "hwy_exit_reset",
     "hwy_abi_version", "hwy_last_error", "hwy_highway_slot_stride", "hwy_highway_reset",
@@ -289,6 +307,7 @@ EXPORTS = (
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
     "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
+    "hwy_lane_keeping_reset", "hwy_lane_keeping_step",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -392,6 +411,11 @@ def load():
     lib.hwy_mcts_recommend.argtypes = [MT, C.c_void_p]
     lib.hwy_mcts_reroot.restype = C.c_int
     lib.hwy_mcts_reroot.argtypes = [MT, C.c_void_p, C.c_void_p, C.c_void_p]
+    LP, LS = C.POINTER(HwyLaneKeepingParams), C.POINTER(HwyLaneKeepingState)
+    lib.hwy_lane_keeping_reset.restype = C.c_int
+    lib.hwy_lane_keeping_reset.argtypes = [LP, LS] + [C.c_void_p] * 4
+    lib.hwy_lane_keeping_step.restype = C.c_int
+    lib.hwy_lane_keeping_step.argtypes = [LP, LS] + [C.c_void_p] * 7
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

@@ -328,3 +328,35 @@ def continuous_intersection_default_config() -> dict:
 
 
 DEFAULTS["intersection-v1"] = continuous_intersection_default_config
+
+
+def lane_keeping_default_config() -> dict:
+    """LaneKeepingEnv.default_config (highway_env/envs/lane_keeping_env.py:25-52) over AbstractEnv's."""
+    import numpy as np
+
+    config = abstract_default_config()
+    update_config(config, {
+        "observation": {
+            "type": "AttributesObservation",
+            "attributes": ["state", "derivative", "reference_state"],
+        },
+        "action": {
+            "type": "ContinuousAction",
+            "steering_range": [-np.pi / 3, np.pi / 3],
+            "longitudinal": False,
+            "lateral": True,
+            "dynamical": True,
+        },
+        "simulation_frequency": 10,
+        "policy_frequency": 10,
+        "state_noise": 0.05,
+        "derivative_noise": 0.05,
+        "screen_width": 600,
+        "screen_height": 250,
+        "scaling": 7,
+        "centering_position": [0.4, 0.5],
+    })
+    return config
+
+
+DEFAULTS["lane-keeping-v0"] = lane_keeping_default_config

@@ -49,6 +49,9 @@ class HostStepper:
         self._h_term, self._h_trunc = pin(env._terminated), pin(env._truncated)
         self.actions = self._h_actions.numpy()
         self.obs, self.reward = self._h_obs.numpy(), self._h_reward.numpy()
+        attributes = getattr(env, "attributes", None)
+        if attributes is not None:  # Dict observation (lane-keeping-v0): views of the one [N, n_attr, ...] buffer
+            self.obs = {a: self.obs[:, k] for k, a in enumerate(attributes)}
         self.terminated, self.truncated = self._h_term.numpy().view(np.bool_), self._h_trunc.numpy().view(np.bool_)
         self._h_obs.copy_(env._obs)
         self._stream = torch.cuda.Stream(device=dev)
@@ -58,7 +61,7 @@ class HostStepper:
             with torch.cuda.graph(self._graph, stream=self._stream):
                 self._d_actions.copy_(self._h_actions, non_blocking=True)
                 obs, reward, term, trunc, _ = env.step(self._d_actions)
-                self._h_obs.copy_(obs, non_blocking=True)
+                self._h_obs.copy_(env._obs if attributes is not None else obs, non_blocking=True)
                 self._h_reward.copy_(env._reward, non_blocking=True)
                 self._h_term.copy_(env._terminated, non_blocking=True)
                 self._h_trunc.copy_(env._truncated, non_blocking=True)

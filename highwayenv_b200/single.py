@@ -23,6 +23,13 @@ except Exception:  # pragma: no cover - gymnasium is not in this image
     _Base = object
 
 
+def _obs_row(obs):
+    """Env 0's observation as numpy; a Dict observation (lane-keeping-v0) as a dict of float64 arrays."""
+    if isinstance(obs, dict):
+        return {k: v[0].cpu().numpy().copy() for k, v in obs.items()}
+    return obs[0].cpu().numpy().copy()
+
+
 def _scalar(v):
     a = v.detach().cpu().numpy() if hasattr(v, "detach") else np.asarray(v)
     a = a.reshape(a.shape[1:]) if a.ndim >= 1 and a.shape[0] == 1 else a
@@ -59,14 +66,14 @@ class SingleEnv(_Base):
 
     def reset(self, *, seed: Optional[int] = None, options: Optional[dict] = None):
         obs, info = self.batched.reset(seed=seed, options=options)
-        return obs[0].cpu().numpy().copy(), self._info(info)
+        return _obs_row(obs), self._info(info)
 
     def step(self, action):
         a = np.asarray(action)
         buf = self.batched._action_buf
         a = a.reshape((1,) + tuple(buf.shape[1:])).astype(np.float32 if buf.dtype.is_floating_point else np.int64)
         obs, reward, terminated, truncated, info = self.batched.step(a)
-        return (obs[0].cpu().numpy().copy(), float(_scalar(reward)), bool(_scalar(terminated)), bool(_scalar(truncated)),
+        return (_obs_row(obs), float(_scalar(reward)), bool(_scalar(terminated)), bool(_scalar(truncated)),
                 self._info(info))
 
     def get_available_actions(self):

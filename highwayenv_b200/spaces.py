@@ -10,7 +10,7 @@ from __future__ import annotations
 import numpy as np
 
 try:  # pragma: no cover - depends on the image
-    from gymnasium.spaces import Box, Discrete  # type: ignore
+    from gymnasium.spaces import Box, Dict, Discrete  # type: ignore
 
     HAVE_GYMNASIUM = True
 except Exception:  # ModuleNotFoundError in this image
@@ -60,9 +60,33 @@ except Exception:  # ModuleNotFoundError in this image
         def __repr__(self):
             return f"Discrete({self.n})"
 
+    class Dict(_Space):
+        """A mapping of named spaces; keys sorted as gymnasium's Dict sorts a plain dict."""
+
+        def __init__(self, spaces, seed=None):
+            super().__init__((), None, seed)
+            self.shape, self.dtype = None, None
+            self.spaces = dict(sorted(dict(spaces).items()))
+
+        def __getitem__(self, key):
+            return self.spaces[key]
+
+        def keys(self):
+            return self.spaces.keys()
+
+        def sample(self):
+            return {k: s.sample() for k, s in self.spaces.items()}
+
+        def contains(self, x):
+            return (isinstance(x, dict) and set(x) == set(self.spaces)
+                    and all(s.contains(x[k]) for k, s in self.spaces.items()))
+
+        def __repr__(self):
+            return "Dict(" + ", ".join(f"{k!r}: {s}" for k, s in self.spaces.items()) + ")"
+
 
 def batch_space(space, n: int):
-    """gymnasium.vector.utils.batch_space for the two space kinds used here."""
+    """gymnasium.vector.utils.batch_space for the space kinds used here."""
     if isinstance(space, Box):
         return Box(
             low=np.broadcast_to(space.low, (n,) + space.shape).copy(),
@@ -76,4 +100,6 @@ def batch_space(space, n: int):
             return MultiDiscrete(np.full((n,), space.n, dtype=np.int64))
         except Exception:
             return Box(low=0, high=space.n - 1, shape=(n,), dtype=np.int64)
+    if isinstance(space, Dict):
+        return Dict({k: batch_space(s, n) for k, s in space.spaces.items()})
     raise TypeError(space)

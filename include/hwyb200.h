@@ -683,6 +683,47 @@ int hwy_mcts_recommend(const HwyMctsTree *t, void *stream);
  * tree. */
 int hwy_mcts_reroot(const HwyMctsTree *t, const int64_t *actions, const uint8_t *done, void *stream);
 
+/* ====================================================================== lane-keeping-v0
+ * LaneKeepingEnv (envs/lane_keeping_env.py): one dynamical BicycleVehicle per env, no traffic, one thread per env.
+ * lanes[0] is ("c", "d", 0), the StraightLane the episode starts on; lanes[1] is ("a", "b", 0), the SineLane queued
+ * after it.  The ego spawns at (x0, y0) with heading0 and speed0, zero lateral speed and yaw rate.
+ * attr[k] in 0 state, 1 derivative, 2 reference_state: the AttributesObservation columns in config order; each
+ * observe draws 4 uniforms per noisy attribute (state, derivative) from the env's stream, in attribute order.
+ * actions [n_envs][longitudinal + lateral] float32: (throttle, steering) of ContinuousAction in that order. */
+#define HWY_LK_MAX_ATTR 3
+typedef struct HwyLaneKeepingParams {
+    int32_t frames;     /* simulation_frequency // policy_frequency (>= 1) */
+    int32_t n_attr;     /* 1..HWY_LK_MAX_ATTR */
+    int32_t attr[HWY_LK_MAX_ATTR];
+    int32_t longitudinal, lateral, act_clip;
+    int32_t max_episode_steps; /* TimeLimit: truncated once this many steps have run since the reset */
+    int32_t autoreset;  /* HWY_AUTORESET_DISABLED or HWY_AUTORESET_SAME_STEP */
+    double dt;          /* 1 / simulation_frequency */
+    double state_noise, derivative_noise;
+    double acc_lo, acc_hi, steer_lo, steer_hi;
+    double x0, y0, heading0, speed0;
+    HwyNetLane lanes[2];
+} HwyLaneKeepingParams;
+typedef struct HwyLaneKeepingState {
+    int32_t n_envs, _pad;
+    double *state;       /* DEVICE [6][n_envs]: x, y, heading, speed, lateral_speed, yaw_rate */
+    int32_t *lane_phase; /* DEVICE [n_envs]: 0 on lanes[0] with lanes[1] queued, 1 on lanes[1] */
+    int32_t *elapsed;    /* DEVICE [n_envs]: steps since the last reset */
+    uint64_t *rng;       /* DEVICE [5][n_envs] */
+} HwyLaneKeepingState;
+/* Reset the envs with mask_a[e] || mask_b[e] (both NULL: every env): the scene of LaneKeepingEnv._reset, then the three
+ * observes of AbstractEnv.reset (two inside define_spaces, whose values are discarded); obs [n_envs][n_attr][4] f64
+ * takes the last one. */
+int hwy_lane_keeping_reset(const HwyLaneKeepingParams *p, const HwyLaneKeepingState *s, const uint8_t *mask_a,
+                           const uint8_t *mask_b, double *obs, void *stream);
+/* One LaneKeepingEnv.step of every env: lane switch, act, observe (of the state before the step), `frames` RK4 frames,
+ * reward 1 - (lat / width)^2 on the env's current lane; terminated = 0, truncated = elapsed >= max_episode_steps.
+ * With autoreset = HWY_AUTORESET_SAME_STEP a truncated env writes its observation to final_obs, is reset as above and
+ * obs takes the reset observation; final_obs rows of the other envs are left as they were. */
+int hwy_lane_keeping_step(const HwyLaneKeepingParams *p, const HwyLaneKeepingState *s, const float *actions,
+                          double *obs, double *final_obs, double *reward, uint8_t *terminated, uint8_t *truncated,
+                          void *stream);
+
 /* Kernel launches issued by the calling thread through this library since load (the
  * `gpu_launches` claim of bench.py). */
 uint64_t hwy_launch_count(void);
