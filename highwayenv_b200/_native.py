@@ -25,6 +25,7 @@ KIND_IDM, KIND_MDP, KIND_VEHICLE = 0, 1, 2
 META_LANE_SHIFT, META_TARGET_SHIFT = 0, 8
 META_CRASHED, META_HAS_IMPACT, META_CHECK_COLLISIONS = 1 << 16, 1 << 17, 1 << 18
 META_KIND_SHIFT, META_PRESENT = 19, 1 << 21
+META_ORDER_SHIFT = 24  # highway: 7 bits, the stored road order (include/hwyb200.h); a checked hint, not state
 AUTORESET_DISABLED, AUTORESET_SAME_STEP = 0, 1
 
 

@@ -258,5 +258,9 @@ __device__ __forceinline__ int meta_set_lane(int m, int l) {
 __device__ __forceinline__ int meta_set_target(int m, int l) {
     return (m & ~(0xff << HWY_META_TARGET_SHIFT)) | (l << HWY_META_TARGET_SHIFT);
 }
+__device__ __forceinline__ int meta_order(int m) { return (m >> HWY_META_ORDER_SHIFT) & 0x7f; }
+__device__ __forceinline__ int meta_set_order(int m, int s) {
+    return (m & ~(0x7f << HWY_META_ORDER_SHIFT)) | (s << HWY_META_ORDER_SHIFT);
+}
 
 }  // namespace hwy

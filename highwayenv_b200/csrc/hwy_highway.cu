@@ -497,6 +497,19 @@ __device__ __forceinline__ void store_vehicle(const HwyHighwayState& S, size_t s
     S.meta[slot] = r.meta;  // delta never changes during a step
 }
 
+// The road order the last launch left in the meta words (HWY_META_ORDER_SHIFT) as the perm / rank of frame G, where
+// build_frame's chain check on the first frame of a launch finds it.  Slot i holds the vehicle of rank i; an entry
+// past the env's vehicles becomes vehicle 0, so that every index the check reads is a vehicle.  rank is the inverse of
+// perm wherever perm is a permutation, the only case in which build_frame reads it.  Callers put a barrier between
+// this and build_frame().
+template <int TPE>
+__device__ __forceinline__ void stage_stored_order(Frame<TPE>& G, int i, int V, int meta) {
+    const int v = meta_order(meta);
+    const int u = v < V ? v : 0;
+    G.perm[i] = (unsigned char)u;
+    G.rank[u] = (unsigned char)i;
+}
+
 // Stage one vehicle into frame F (plain stores) and clear the words of F that build_frame fills
 // with atomics (DENSE: the caller does, clear_masks).  Callers put a barrier between publish() and build_frame().
 template <int TPE, bool LINEAR = false, bool DENSE = false>
@@ -594,9 +607,9 @@ __device__ __noinline__ void pair_sat(const Frame<TPE>& F, int a, int b, double 
                           F.v[b] * F.s[b] * dt, inter, will, trx, try_);
 }
 
-// Rank of vehicle i along the road by counting (O(V) per thread), out of line: it runs on the first frame of a launch
-// and when the previous order broke (see build_frame), and its unrolled loops are 8 KB of code that the per-substep
-// loop should not carry.  Returns rank | tie << 8.
+// Rank of vehicle i along the road by counting (O(V) per thread), out of line: it runs only when the previous order
+// broke (see build_frame), and its unrolled loops are 8 KB of code that the per-substep loop should not carry.
+// Returns rank | tie << 8.
 template <int TPE>
 __device__ __noinline__ int rank_count(const Frame<TPE>& F, int V, int i, bool active) {
     const double si = active ? F.ls[i] : 0.0;
@@ -723,34 +736,37 @@ __device__ __noinline__ int rank_repair(const Frame<TPE>& F, const Frame<TPE>& p
 template <int TPE, bool DENSE>
 __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared<TPE>& sm, Frame<TPE>& F,
                                             int i, bool active, bool aligned, const VehicleRegs& r,
-                                            double dt, bool do_sweep, bool pruned, const Frame<TPE>* prev) {
+                                            double dt, bool do_sweep, bool do_masks, bool pruned,
+                                            const Frame<TPE>& prev) {
     const int V = P.n_vehicles;
     const int wie = i >> 5;  // warp within the env (TPE-thread segments)
     const int lane = meta_lane(r.meta), tgt = meta_target(r.meta);
     // -- rank along the road (s, slot) and tie detection.  Float keys first: rounding to float
     // is monotone, so fu < fi implies su < si; only equal float keys need the doubles.
     int rank = 0;
-    // The order along the road rarely changes within one substep: with the previous frame of the same launch at hand
-    // (`prev`, uniform), every warp checks the whole chain key[perm[k-1]] < key[perm[k]] under the previous permutation
-    // of each env segment it holds, one with TPE-thread segments (V - 1 float comparisons spread over its 32 lanes, no
-    // communication between the warps: each warp of an env reaches the same verdict).  A strictly increasing chain of
-    // float keys is a strictly increasing chain of the doubles they were rounded from, so the ranks are the previous
-    // ones and there is neither a tie nor an ambiguity — the O(V) scan per thread (14 % of the kernel's instructions
-    // at V = 51) runs only when some pair swapped or drew level.
+    // The order along the road rarely changes within one substep: `prev` holds the previous frame of the same launch,
+    // or on the first frame the order the last launch left in the meta words (stage_stored_order).  Every warp checks
+    // the whole chain key[perm[k-1]] < key[perm[k]] under that permutation of each env segment it holds, one with
+    // TPE-thread segments (V - 1 float comparisons spread over its 32 lanes, no communication between the warps: each
+    // warp of an env reaches the same verdict).  A strictly increasing chain of float keys is a strictly increasing
+    // chain of the doubles they were rounded from, so the ranks are the stored ones and there is neither a tie nor an
+    // ambiguity — the O(V) scan per thread (14 % of the kernel's instructions at V = 51) runs only when some pair
+    // swapped or drew level.  The chain also proves that the V entries are V distinct vehicles, so the stored order
+    // needs no other check: whatever it came from, a permutation that orders the current keys strictly is their order.
     bool reuse = false;
-    if (prev && !DENSE) {
+    if constexpr (!DENSE) {
         bool ok = true;
 #pragma unroll 1
-        for (int k = (i & 31) + 1; k < V; k += 32) ok = ok && (F.lsf[prev->perm[k - 1]] < F.lsf[prev->perm[k]]);
+        for (int k = (i & 31) + 1; k < V; k += 32) ok = ok && (F.lsf[prev.perm[k - 1]] < F.lsf[prev.perm[k]]);
         reuse = __all_sync(0xffffffffu, ok);
-    } else if (prev) {
+    } else {
         int mine, s = 0;
 #pragma unroll 1
         for (uint32_t lead = segment_leads(i, active, mine); lead; lead &= lead - 1, ++s) {
             // env of segment s: the envs of a block are consecutive EnvShared records
             const ptrdiff_t d = (ptrdiff_t)(s - mine) * (ptrdiff_t)sizeof(EnvShared<TPE>);
             const Frame<TPE>& Fs = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(&F) + d);
-            const Frame<TPE>& Ps = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(prev) + d);
+            const Frame<TPE>& Ps = *reinterpret_cast<const Frame<TPE>*>(reinterpret_cast<const char*>(&prev) + d);
             bool ok = true;
 #pragma unroll 1
             for (int k = lane_id() + 1; k < V; k += 32)
@@ -762,20 +778,20 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     bool tie = false;
     if constexpr (!DENSE) {
         if (reuse) {
-            rank = active ? prev->rank[i] : 0;
+            rank = active ? prev.rank[i] : 0;
         } else {
             // (the repair pays for itself only where the count is long, so only the 128-slot kernel uses it)
-            int rt = (TPE >= 128 && prev) ? rank_repair<TPE, DENSE>(F, *prev, V, i, active) : -1;
-            if (rt < 0) rt = rank_count(F, V, i, active);  // first frame of a launch, ties, or more than isolated swaps
+            int rt = TPE >= 128 ? rank_repair<TPE, DENSE>(F, prev, V, i, active) : -1;
+            if (rt < 0) rt = rank_count(F, V, i, active);  // no usable stored order, ties, or more than isolated swaps
             rank = rt & 0xff;
             tie = (rt >> 8) != 0;
         }
     } else {
         // the verdict differs between the segments of a warp, and the repair is warp-wide
         int rt = -1;
-        if (TPE >= 128 && prev && __any_sync(0xffffffffu, !reuse)) rt = rank_repair<TPE, DENSE>(F, *prev, V, i, active);
+        if (TPE >= 128 && __any_sync(0xffffffffu, !reuse)) rt = rank_repair<TPE, DENSE>(F, prev, V, i, active);
         if (reuse) {
-            rank = active ? prev->rank[i] : 0;
+            rank = active ? prev.rank[i] : 0;
         } else if (active) {
             if (rt < 0) rt = rank_count(F, V, i, active);
             rank = rt & 0xff;
@@ -786,34 +802,39 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
         F.perm[rank] = (unsigned char)i;
         F.rank[i] = (unsigned char)rank;
         if (tie || !aligned) F.slow = 1;
+    }
+    // -- the membership masks serve Road.act only, which the last frame of a launch does not run (do_masks, uniform)
+    if (do_masks) {
+        if (active) {
+#pragma unroll 1
+            for (int l = 0; l < P.lanes_count; ++l) {
+                double s_l, lat_l;
+                lane_local(P.lanes[l], r.x, r.y, s_l, lat_l);
+                if (lane_on(P.lanes[l], s_l, lat_l, 1.0)) atomicOr(&F.smask[l][rank >> 5], 1u << (rank & 31));
+            }
+        }
+        // slot-ordered masks by ballot
+        const bool is_idm = meta_kind(r.meta) == HWY_KIND_IDM;
 #pragma unroll 1
         for (int l = 0; l < P.lanes_count; ++l) {
-            double s_l, lat_l;
-            lane_local(P.lanes[l], r.x, r.y, s_l, lat_l);
-            if (lane_on(P.lanes[l], s_l, lat_l, 1.0)) atomicOr(&F.smask[l][rank >> 5], 1u << (rank & 31));
+            uint32_t b_lane = __ballot_sync(0xffffffffu, active && lane == l);
+            uint32_t b_tgt = __ballot_sync(0xffffffffu, active && tgt == l);
+            if constexpr (DENSE) {
+                segment_or(F.lane_is[l], b_lane, i, V);
+                segment_or(F.tm[l], b_tgt, i, V);
+            } else if ((i & 31) == 0) {
+                F.lane_is[l][wie] = b_lane;
+                F.tm[l][wie] = b_tgt;
+            }
         }
+        // superset of the vehicles whose MOBIL decision may fire in the coming act (the crashed
+        // flag may still be stale here; crashed vehicles never fire, so this only over-approximates)
+        uint32_t b_fired = __ballot_sync(0xffffffffu, active && is_idm && lane == tgt && P.lane_change_delay < r.timer);
+        if constexpr (DENSE)
+            segment_or(F.fired, b_fired, i, V);
+        else if ((i & 31) == 0)
+            F.fired[wie] = b_fired;
     }
-    // -- slot-ordered masks by ballot
-    const bool is_idm = meta_kind(r.meta) == HWY_KIND_IDM;
-#pragma unroll 1
-    for (int l = 0; l < P.lanes_count; ++l) {
-        uint32_t b_lane = __ballot_sync(0xffffffffu, active && lane == l);
-        uint32_t b_tgt = __ballot_sync(0xffffffffu, active && tgt == l);
-        if constexpr (DENSE) {
-            segment_or(F.lane_is[l], b_lane, i, V);
-            segment_or(F.tm[l], b_tgt, i, V);
-        } else if ((i & 31) == 0) {
-            F.lane_is[l][wie] = b_lane;
-            F.tm[l][wie] = b_tgt;
-        }
-    }
-    // superset of the vehicles whose MOBIL decision may fire in the coming act (the crashed
-    // flag may still be stale here; crashed vehicles never fire, so this only over-approximates)
-    uint32_t b_fired = __ballot_sync(0xffffffffu, active && is_idm && lane == tgt && P.lane_change_delay < r.timer);
-    if constexpr (DENSE)
-        segment_or(F.fired, b_fired, i, V);
-    else if ((i & 31) == 0)
-        F.fired[wie] = b_fired;
 
     // -- collision sweep, pass 1: every gated pair once.  A pair with exactly one
     // check_collisions side is taken by the other side's thread (so the controlled vehicle's
@@ -1166,8 +1187,10 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
         r.timer = timer;
         r.delta = delta;
         r.imp_x = r.imp_y = 0.0;
+        // road order: on the x-aligned highway the spawn positions increase with the slot
         r.meta = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) |
-                 (cc ? HWY_META_CHECK_COLLISIONS : 0) | (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT;
+                 (cc ? HWY_META_CHECK_COLLISIONS : 0) | (kind << HWY_META_KIND_SHIFT) | HWY_META_PRESENT |
+                 ((simple_geometry ? i : 0) << HWY_META_ORDER_SHIFT);
     }
 }
 

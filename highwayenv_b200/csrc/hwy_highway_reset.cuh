@@ -72,9 +72,10 @@
         tt[base + v] = make_double2(target_speed, timer);
         imp[base + v] = make_double2(0.0, 0.0);
         S.delta[base + v] = delta;
+        // road order: with aligned lanes the spawn positions increase with the slot
         S.meta[base + v] = (lane << HWY_META_LANE_SHIFT) | (lane << HWY_META_TARGET_SHIFT) |
                            (cc ? HWY_META_CHECK_COLLISIONS : 0) | (kind << HWY_META_KIND_SHIFT) |
-                           HWY_META_PRESENT;
+                           HWY_META_PRESENT | ((aligned ? v : 0) << HWY_META_ORDER_SHIFT);
     }
     S.speed_index[e] = ego_speed_index;
     S.time[e] = 0.0;

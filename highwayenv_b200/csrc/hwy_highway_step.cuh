@@ -79,6 +79,9 @@
     // already costs one pre-check per thread
     const bool pruned = P.others_check_collisions != 0;
     int p = 1;
+    // frame 0 takes its ranks from the order the last launch stored, once build_frame has checked it (sm.f[1] is the
+    // previous frame of frame 0; the barrier after frame 0's publish orders these stores)
+    if (active) stage_stored_order(sm.f[1], i, V, r.meta);
     PHASE_INIT();
     PHASE_MARK(0);  // load + static masks
 
@@ -88,16 +91,17 @@
         p ^= 1;
         Frame<TPE>& F = sm.f[p];
         publish<TPE, LINEAR, DENSE>(P, F, i, active, r);
-        if (DENSE && active) clear_masks(F, i, V);
+        const bool acts = frame < frames;  // the last frame only feeds the collision sweep and the epilogue
+        if (DENSE && active && acts) clear_masks(F, i, V);
         PHASE_MARK(1);  // publish
         env_sync<TPE>();
         PHASE_MARK(2);  // barrier after publish
         if (i < NW) sm.mid[i] = sm.ok_left[i] = sm.ok_right[i] = 0;  // all readers are past phase B
         if (i == 0) sm.n_items = 0;
         // frame 0: masks only — the sweep of the stored state ran at the end of the substep that
-        // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).
-        build_frame<TPE, DENSE>(P, sm, F, i, active, aligned, r, dt, frame > 0, pruned,
-                                frame > 0 ? &sm.f[p ^ 1] : nullptr);
+        // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).  The last frame: ranks and
+        // the sweep, no masks.
+        build_frame<TPE, DENSE>(P, sm, F, i, active, aligned, r, dt, frame > 0, acts, pruned, sm.f[p ^ 1]);
         PHASE_MARK(3);  // ranks, masks, sweep pass 1
         if (pruned && frame > 0) {  // uniform over the grid
             env_sync_phase<TPE, 3>();
@@ -411,6 +415,8 @@
     }
 
     PHASE_MARK(11);
+    // the final frame's road order goes back with the state, for frame 0 of the next launch
+    if (active) r.meta = meta_set_order(r.meta, sm.f[p].perm[i]);
     if (substeps_only) {  // uniform over the grid
         if (active && env_ok) store_vehicle(S, slot, r);
         return;

@@ -46,6 +46,11 @@ extern "C" {
 #define HWY_META_CHECK_COLLISIONS (1 << 18)
 #define HWY_META_KIND_SHIFT 19        /* 2 bits */
 #define HWY_META_PRESENT (1 << 21)
+/* highway family only, 7 bits: the slot of the env's vehicle of rank v along the road (v = this slot's index) as of
+ * the last frame a highway kernel built, or after a spawn whose positions increase with the slot.  A hint for the next
+ * step's first frame, which checks it against the positions before using it: any value is safe, and the reset value
+ * 0 in every slot (what a state written from the host has) just means "recount". */
+#define HWY_META_ORDER_SHIFT 24
 /* kinds (2 bits): 0 IDMVehicle, 1 MDPVehicle, 2 plain Vehicle (ContinuousAction ego), 3 Obstacle — a static 2 x 2 m
  * road object (vehicle/objects.py:213-220); road.objects occupy the slots after the vehicles */
 #define HWY_KIND_OBSTACLE 3
