@@ -42,6 +42,9 @@ REGISTRY = {
     "intersection-multi-agent-v2": "highwayenv_b200.envs.intersection_env:BatchedConnectedLaneMultiAgentIntersectionEnv",
     # one dynamical BicycleVehicle on a sine lane, Dict observation, TimeLimit(max_episode_steps=200)
     "lane-keeping-v0": "highwayenv_b200.envs.lane_keeping_env:BatchedLaneKeepingEnv",
+    # a plain Vehicle steered round a two-lane track with IDM traffic; OccupancyGrid (presence, on_road)
+    "racetrack-v0": "highwayenv_b200.envs.racetrack_env:BatchedRacetrackEnv",
+    "racetrack-v1": "highwayenv_b200.envs.racetrack_env:BatchedConnectedLaneRacetrackEnv",
 }
 
 

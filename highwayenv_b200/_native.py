@@ -211,6 +211,13 @@ class HwyRoundaboutSpawn(C.Structure):
     ]
 
 
+class HwyRacetrackParams(C.Structure):
+    _fields_ = [("other_vehicles", C.c_int32), ("terminate_off_road", C.c_int32), ("lane_ab", C.c_int32),
+                ("lane_bc", C.c_int32), ("n_from_nodes", C.c_int32), ("_pad", C.c_int32),
+                ("lane_centering_cost", C.c_double), ("lane_centering_reward", C.c_double),
+                ("action_reward", C.c_double), ("collision_reward", C.c_double), ("on_road_reward", C.c_double)]
+
+
 FEAT_ON_ROAD, FEAT_UNKNOWN = 13, 14
 HWY_NET_MAX_ROUTE = 16
 
@@ -308,7 +315,7 @@ EXPORTS = (
     "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
     "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
-    "hwy_lane_keeping_reset", "hwy_lane_keeping_step",
+    "hwy_lane_keeping_reset", "hwy_lane_keeping_step", "hwy_racetrack_reset", "hwy_racetrack_step",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -417,6 +424,11 @@ def load():
     lib.hwy_lane_keeping_reset.argtypes = [LP, LS] + [C.c_void_p] * 4
     lib.hwy_lane_keeping_step.restype = C.c_int
     lib.hwy_lane_keeping_step.argtypes = [LP, LS] + [C.c_void_p] * 7
+    RP = C.POINTER(HwyRacetrackParams)
+    lib.hwy_racetrack_reset.restype = C.c_int
+    lib.hwy_racetrack_reset.argtypes = [NP, NG, RP, NS] + [C.c_void_p] * 5
+    lib.hwy_racetrack_step.restype = C.c_int
+    lib.hwy_racetrack_step.argtypes = [NP, NG, RP, NS, C.c_void_p, C.c_int] + [C.c_void_p] * 7
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

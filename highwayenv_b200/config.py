@@ -360,3 +360,43 @@ def lane_keeping_default_config() -> dict:
 
 
 DEFAULTS["lane-keeping-v0"] = lane_keeping_default_config
+
+
+def racetrack_default_config() -> dict:
+    """RacetrackEnv.default_config (highway_env/envs/racetrack_env.py:28-64) over AbstractEnv's."""
+    config = abstract_default_config()
+    update_config(config, {
+        "observation": {
+            "type": "OccupancyGrid",
+            "features": ["presence", "on_road"],
+            "grid_size": [[-18, 18], [-18, 18]],
+            "grid_step": [3, 3],
+            "as_image": False,
+            "align_to_vehicle_axes": True,
+        },
+        "action": {
+            "type": "ContinuousAction",
+            "longitudinal": False,
+            "lateral": True,
+            "target_speeds": [0, 5, 10],
+        },
+        "simulation_frequency": 15,
+        "policy_frequency": 5,
+        "duration": 300,
+        "collision_reward": -1,
+        "lane_centering_cost": 4,
+        "lane_centering_reward": 1,
+        "action_reward": -0.3,
+        "controlled_vehicles": 1,
+        "other_vehicles": 1,
+        "screen_width": 600,
+        "screen_height": 600,
+        "centering_position": [0.5, 0.5],
+        "speed_limit": 10.0,
+        "terminate_off_road": True,
+    })
+    return config
+
+
+DEFAULTS["racetrack-v0"] = racetrack_default_config
+DEFAULTS["racetrack-v1"] = _connected(racetrack_default_config)

@@ -2264,6 +2264,167 @@ two_way_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* 
     store_env_tail(S, rng, e, SP.ego_speed_index, P.n_vehicles, g);
 }
 
+// ------------------------------------------------------------------ racetrack-v0 / v1 (envs/racetrack_env.py)
+// RacetrackEnv._make_vehicles (:374-425), one env per thread: the plain Vehicle on ("a","b",integers(2)) at
+// uniform(20, 50) and the lane's speed limit; with other_vehicles > 0 the IDMVehicle on ("b","c", the ego's lane id) at
+// uniform(0, length of ("b","c",0)), speed 6 + uniform(0, 3); then integers(other_vehicles) attempts on
+// random_lane_index, each dropped when it lands closer than 20 m to a vehicle already placed.  No randomize_behavior:
+// DELTA stays 4.  The slots past the population are cleared.
+__global__ void __launch_bounds__(128)
+racetrack_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
+                       const __grid_constant__ HwyRacetrackParams RP, const __grid_constant__ HwyNetState S,
+                       uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
+    Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
+    const size_t base = (size_t)e * S.vp;
+    double xs[HWY_NET_GROUP], ys[HWY_NET_GROUP];
+    int n = 0;
+    // make_on_lane (vehicle/objects.py:68-90) into slot n; `check`: the 20 m test against the vehicles placed so far
+    auto place = [&](int lane_index, double lon, double speed, int kind, bool check) {
+        const HwyNetLane& L = graph->lanes[lane_index];
+        double px, py;
+        lane_position(L, lon, 0.0, px, py);
+        if (check)
+            for (int v = 0; v < n; ++v)
+                if (norm2(px - xs[v], py - ys[v]) < 20) return;
+        const double heading = lane_heading_at(L, lon);
+        const int lane = closest_lane(graph, px, py, heading);
+        // a plain Vehicle starts with the action {acceleration: 0, steering: 0} in its (target_speed, timer) pair
+        store_vehicle(P, S, base + n, px, py, heading, speed, kind == HWY_KIND_IDM ? speed : 0.0, 4.0, lane, lane, kind);
+        S.route_len[base + n] = 0;
+        xs[n] = px;
+        ys[n] = py;
+        ++n;
+    };
+    const int ego_id = g.choice(2);
+    const double ego_lon = g.uniform(20.0, 50.0);
+    place(RP.lane_ab + ego_id, ego_lon, graph->lanes[RP.lane_ab + ego_id].speed_limit, HWY_KIND_VEHICLE, false);
+    if (RP.other_vehicles > 0) {
+        const double lon = g.uniform(0.0, graph->lanes[RP.lane_bc].length);
+        const double speed = 6.0 + g.uniform(0.0, 3.0);
+        place(RP.lane_bc + ego_id, lon, speed, HWY_KIND_IDM, false);
+        const int extra = g.choice(RP.other_vehicles);
+        for (int k = 0; k < extra; ++k) {
+            // RoadNetwork.random_lane_index (road/road.py:364-368): choice(graph), choice(graph[_from]), integers(lanes)
+            const int f = g.choice(RP.n_from_nodes);
+            const int road = graph->succ[f][g.choice(graph->succ_count[f])];
+            const int lane_index = road + g.choice(graph->lanes[road].road_count);
+            const double lon_k = g.uniform(0.0, graph->lanes[lane_index].length);
+            const double speed_k = 6.0 + g.uniform(0.0, 3.0);
+            place(lane_index, lon_k, speed_k, HWY_KIND_IDM, true);
+        }
+    }
+    for (int v = n; v < S.vp; ++v) {
+        const size_t k = base + v;
+        reinterpret_cast<double2*>(S.pos)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.hs)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.tt)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.imp)[k] = make_double2(0.0, 0.0);
+        S.delta[k] = 0.0;
+        S.meta[k] = 0;
+        S.route_len[k] = 0;
+    }
+    store_env_tail(S, rng, e, 0, n, g);
+}
+
+// One RacetrackEnv.step per env (n_substeps == 0), or n_substeps x (Road.act; Road.step) alone: the network substep
+// with a plain ego (PLAIN, no RegulatedRoad), then the observation and the racetrack reward (:66-92).  Its own
+// instantiation of the substep, so that the other network kernels are compiled as before.
+template <int G>
+__global__ void __launch_bounds__(kStepThreads, 1)
+racetrack_step_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
+                      const __grid_constant__ HwyRacetrackParams RP, const __grid_constant__ HwyNetState S,
+                      const float* __restrict__ action, int n_substeps, float* __restrict__ obs,
+                      double* __restrict__ reward, uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
+                      double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    GraphShared& g = *reinterpret_cast<GraphShared*>(smem_raw);
+    EnvStage<G, false>* stages =
+        reinterpret_cast<EnvStage<G, false>*>(smem_raw + ((sizeof(GraphShared) + 15) & ~size_t(15)));
+    const int kEnvs = blockDim.x / G;
+    if (blockIdx.x * kEnvs >= S.n_envs) return;  // uniform per block
+    stage_graph(g, graph);
+    const int sub = threadIdx.x / G, i = threadIdx.x % G;
+    const int idx = blockIdx.x * kEnvs + sub;
+    const bool env_ok = idx < S.n_envs;  // the spare groups of the last block ride along on the last env
+    const int e = env_ok ? idx : S.n_envs - 1;
+    EnvStage<G, false>& st = stages[sub];
+    Regs r;
+    load_env(P, g, S, st, e, i, r);
+    // Vehicle.action persists between steps (kinematics.py:119-128); the state keeps it in the plain ego's
+    // (target_speed, timer) pair.  A plain Vehicle has no target speed: IDMVehicle.acceleration reads 0 for it
+    // (behavior.py:165-170), so the stage holds 0.
+    const bool plain = i < st.count && meta_kind(r.meta) == HWY_KIND_VEHICLE;
+    double act_accel = 0.0, act_steer = 0.0;
+    if (plain) {
+        act_accel = r.target_speed;
+        act_steer = r.timer;
+        r.target_speed = r.timer = 0.0;
+        st.ts[i] = 0.0;
+    }
+    group_sync<G>();
+    const bool policy_step = n_substeps == 0;
+    const int frames = policy_step ? P.simulation_frequency / P.policy_frequency : n_substeps;
+    const double dt = 1.0 / P.simulation_frequency;
+    const float* act_f = policy_step ? action + 2 * (size_t)e : nullptr;
+    for (int frame = 0; frame < frames; ++frame)
+        substep<G, false, true>(P, g, st, i, r, act_accel, act_steer, dt, -1, nullptr, frame == 0 ? act_f : nullptr);
+    group_sync<G>();
+    if (policy_step) {
+        observe_any(P, g, st, st.count, i, obs + (size_t)e * obs_size(P));
+        if (i == st.ego && i < st.count && env_ok) {
+            // _rewards (:72-83) on Vehicle.lane: the closest lane (heading included) after the last substep
+            const HwyNetLane& L = g.lanes[st.lane[i]];
+            const double lat = st.own_lat[i];
+            const bool on_road = lane_on(L, st.own_s[i], lat, 0.0);
+            const bool crashed = (r.meta & HWY_META_CRASHED) != 0;
+            const double centering = 1.0 / (1.0 + RP.lane_centering_cost * (lat * lat));
+            // np.linalg.norm of the float32 action as passed (before the clip); a missing axis is staged as 0 and
+            // adds an exact 0.  NEP 50 keeps config["action_reward"] * it in float32
+            const float a0 = act_f[0], a1 = act_f[1];
+            const float norm = __fsqrt_rn(__fadd_rn(__fmul_rn(a0, a0), __fmul_rn(a1, a1)));
+            // sum() of the weighted terms (:66-70).  StraightLane.local_coordinates returns python floats
+            // (road/lane.py:209-213), and a python float or int added to the float32 action term is weak: the partial
+            // sums through the collision term stay float32.  CircularLane's are np.float64 (:355-362): float64 sums.
+            // on_road's term (int64 or float64) is float64.
+            const float action_term = __fmul_rn((float)RP.action_reward, norm);
+            const double collision_term = RP.collision_reward * (crashed ? 1.0 : 0.0);
+            double rew;
+            if (L.type == HWY_LANE_STRAIGHT) {
+                float sum32 = __fadd_rn((float)(RP.lane_centering_reward * centering), action_term);
+                rew = (double)__fadd_rn(sum32, (float)collision_term);
+            } else {
+                rew = (RP.lane_centering_reward * centering + (double)action_term) + collision_term;
+            }
+            rew = rew + RP.on_road_reward * (on_road ? 1.0 : 0.0);
+            rew = lmap(rew, RP.collision_reward, 1.0, 0.0, 1.0);
+            rew *= on_road ? 1.0 : 0.0;
+            if (S.reward_terms) {
+                double* rt = S.reward_terms + (size_t)e * HWY_REWARD_TERMS;
+                rt[0] = centering;
+                rt[1] = (double)norm;
+                rt[2] = crashed ? 1.0 : 0.0;
+                rt[3] = on_road ? 1.0 : 0.0;
+                rt[4] = 0.0;
+            }
+            const double t = S.time[e] + 1.0 / P.policy_frequency;
+            S.time[e] = t;
+            reward[e] = rew;
+            terminated[e] = (uint8_t)(crashed || (RP.terminate_off_road && !on_road));
+            truncated[e] = (uint8_t)(t >= P.duration);
+            if (info_speed) info_speed[e] = r.speed;
+            if (info_crashed) info_crashed[e] = (uint8_t)crashed;
+        }
+        group_sync<G>();
+    }
+    if (plain) {  // Vehicle.clip_actions edits the action dict in place (kinematics.py:155-168): keep what it left
+        r.target_speed = act_accel;
+        r.timer = act_steer;
+    }
+    if (env_ok) store_env(S, st, e, i, i < st.count ? i : -1, r);
+}
+
 }  // namespace hwynet
 
 // ====================================================================== C ABI
@@ -2454,6 +2615,18 @@ int scripted_reset(K kernel, const char* name, int threads_per_env, const HwyNet
     if (check_launch(name)) return 1;
     return obs ? observe_dispatch(p, graph, s, mask_a, mask_b, obs, st) : 0;
 }
+int validate_racetrack(const HwyNetParams* p, const HwyRacetrackParams* rp, const HwyNetState* s) {
+    if (!rp) return fail("%s", "null racetrack params");
+    if (s->vp != HWY_NET_GROUP || !s->count) return fail("%s", "racetrack: slot stride 8 and the count buffer");
+    if (rp->other_vehicles < 0 || rp->other_vehicles > HWY_NET_GROUP - 1)
+        return fail("%s", "racetrack: other_vehicles out of range (0..7)");
+    if (rp->lane_ab < 0 || rp->lane_ab + 1 >= HWY_NET_MAX_LANES || rp->lane_bc < 0 || rp->lane_bc + 1 >= HWY_NET_MAX_LANES)
+        return fail("%s", "racetrack: lane index out of range");
+    if (rp->n_from_nodes < 1 || rp->n_from_nodes > HWY_NET_MAX_NODES) return fail("%s", "racetrack: n_from_nodes out of range");
+    if (p->action_type != 1 || p->dynamical) return fail("%s", "racetrack: ContinuousAction with a plain Vehicle only");
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2595,6 +2768,30 @@ int hwy_two_way_reset(const HwyNetParams* p, const HwyNetGraph* graph, const Hwy
     if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "two-way-v0: 6 vehicles on 8 slots");
     return scripted_reset(hwynet::two_way_reset_kernel, "two_way_reset_kernel", 1,
                           p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
+}
+
+int hwy_racetrack_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRacetrackParams* rp,
+                        const HwyNetState* s, uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs,
+                        void* stream) {
+    if (validate_net(p, graph, s) || validate_racetrack(p, rp, s)) return 1;
+    if (!rng) return fail("%s", "null rng");
+    return scripted_reset(hwynet::racetrack_reset_kernel, "racetrack_reset_kernel", 1,
+                          p, graph, rp, s, rng, mask_a, mask_b, obs, stream);
+}
+
+int hwy_racetrack_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRacetrackParams* rp,
+                       const HwyNetState* s, const float* action, int n_substeps, float* obs, double* reward,
+                       uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
+                       void* stream) {
+    if (validate_net(p, graph, s) || validate_racetrack(p, rp, s)) return 1;
+    if (n_substeps < 0) return fail("%s", "n_substeps < 0");
+    if (n_substeps == 0 && (!action || !obs || !reward || !terminated || !truncated)) return fail("%s", "null pointer");
+    constexpr int G = HWY_NET_GROUP;
+    const StepPlan plan = step_plan<G, false>(s->n_envs);
+    if (configure_smem(hwynet::racetrack_step_kernel<G>, stage_smem_bytes<G, false>(hwynet::kStepThreads / G))) return 1;
+    hwynet::racetrack_step_kernel<G><<<plan.blocks, plan.threads, plan.smem, (cudaStream_t)stream>>>(
+        *p, graph, *rp, *s, action, n_substeps, obs, reward, terminated, truncated, info_speed, info_crashed);
+    return check_launch("racetrack_step_kernel");
 }
 
 int hwy_network_substeps(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, const uint8_t* mask,

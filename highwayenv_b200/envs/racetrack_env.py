@@ -1,0 +1,247 @@
+"""Batched racetrack-v0 / racetrack-v1 on the H100 backend.
+
+Host-side mirror of the reference's ``RacetrackEnv`` (highway_env/envs/racetrack_env.py:15-425): a closed two-lane
+track of 9 roads (straight and circular, width 5, speed limit 10), one controlled plain ``Vehicle`` steered through
+``ContinuousAction`` (lateral, optionally longitudinal), an ``IDMVehicle`` ahead of it on ("b", "c") and up to
+``other_vehicles - 1`` more on random lanes, each dropped when it spawns within 20 m of one already placed.  The
+default observation is a 12 x 12 OccupancyGrid (presence, on_road) aligned with the vehicle, observed by the standalone
+grid kernel; Kinematics is written by the step kernel itself.
+
+Stepping runs in ``hwy_racetrack_step`` (include/hwyb200.h) on the 8-slot network state: the network kernels' substep
+with a plain ego, then the racetrack reward (:66-83), termination (crash, or off road with ``terminate_off_road``) and
+truncation at ``duration``.  Resets run in ``hwy_racetrack_reset`` from each env's numpy stream, in the reference's
+draw order (:374-425).  The plain Vehicle's action dict persists between steps (kinematics.py:119-128): the state
+keeps it in the ego's (target_speed, timer) pair as (acceleration, steering), which ``road_substeps`` replays.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from .. import _native as N
+from ..road.network import NetworkTable
+from ..spaces import Box, batch_space
+from .common.action import ContinuousAction
+from .common.observation import KinematicObservation, OccupancyGridObservation, select_network_observation
+from .common.vector_env import BatchedNetworkEnv
+
+# LineType (road/lane.py:12-20): NONE 0, STRIPED 1, CONTINUOUS 2
+_N, _S, _C = 0, 1, 2
+
+
+def make_racetrack_network() -> NetworkTable:
+    """RacetrackEnv._make_road (racetrack_env.py:94-358), lanes in the reference's insertion order.  Some arcs end at
+    different angles on their two lanes (136 / 137 deg, 170 / 165 deg, 56 / 58 deg, 240-270 / 238-268 deg); they are
+    copied as they are."""
+    net = NetworkTable()
+    d = np.deg2rad
+
+    def straight(f, t, start, end, lt):
+        net.add_straight(f, t, start, end, width=5, speed_limit=10.0)
+        net._graph[f][t][-1]["line_types"] = list(lt)
+
+    def arc(f, t, center, radius, a0, a1, clockwise, lt):
+        net.add_circular(f, t, center, radius, d(a0), d(a1), clockwise=clockwise, width=5, speed_limit=10.0)
+        net._graph[f][t][-1]["line_types"] = list(lt)
+
+    straight("a", "b", [42, 0], [100, 0], (_C, _S))
+    straight("a", "b", [42, 5], [100, 5], (_S, _C))
+    arc("b", "c", [100, -20], 20, 90, -1, False, (_C, _N))
+    arc("b", "c", [100, -20], 20 + 5, 90, -1, False, (_S, _C))
+    straight("c", "d", [120, -20], [120, -30], (_C, _N))
+    straight("c", "d", [125, -20], [125, -30], (_S, _C))
+    arc("d", "e", [105, -30], 15, 0, -181, False, (_C, _N))
+    arc("d", "e", [105, -30], 15 + 5, 0, -181, False, (_S, _C))
+    arc("e", "f", [70, -30], 15 + 5, 0, 136, True, (_C, _S))
+    arc("e", "f", [70, -30], 15, 0, 137, True, (_N, _C))
+    straight("f", "g", [55.7, -15.7], [35.7, -35.7], (_C, _N))
+    straight("f", "g", [59.3934, -19.2], [39.3934, -39.2], (_S, _C))
+    arc("g", "h", [18.1, -18.1], 25, 315, 170, False, (_C, _N))
+    arc("g", "h", [18.1, -18.1], 25 + 5, 315, 165, False, (_S, _C))
+    arc("h", "i", [18.1, -18.1], 25, 170, 56, False, (_C, _N))
+    arc("h", "i", [18.1, -18.1], 25 + 5, 170, 58, False, (_S, _C))
+    arc("i", "a", [43.2, 23.4], 18.5 + 5, 240, 270, True, (_C, _S))
+    arc("i", "a", [43.2, 23.4], 18.5, 238, 268, True, (_N, _C))
+    net.finalize()
+    return net
+
+
+_HOST_NET = None
+
+
+def _host_network() -> NetworkTable:
+    global _HOST_NET
+    if _HOST_NET is None:
+        _HOST_NET = make_racetrack_network()
+    return _HOST_NET
+
+
+def racetrack_params(cfg: dict, env_id: str = "racetrack-v0") -> dict:
+    """The kernel parameters of a racetrack config (HwyNetParams, HwyRacetrackParams) and its action / observation
+    plugins; raises for what the accelerated path does not run, before anything touches the device."""
+    act, obs = cfg["action"], cfg["observation"]
+    if act["type"] != "ContinuousAction":
+        raise NotImplementedError(f"action type {act['type']!r} on {env_id} (ContinuousAction only)")
+    if int(cfg["controlled_vehicles"]) != 1:
+        raise NotImplementedError(f"controlled_vehicles > 1 on {env_id}")
+    if obs["type"] not in ("OccupancyGrid", "Kinematics"):
+        raise NotImplementedError(f"observation type {obs['type']!r} on {env_id} (OccupancyGrid, Kinematics)")
+    other = int(cfg["other_vehicles"])
+    if other > N.HWY_NET_GROUP - 1:
+        raise NotImplementedError(f"other_vehicles > {N.HWY_NET_GROUP - 1}: 8 slots hold the ego, the front "
+                                  "vehicle and at most 6 more")
+    if other < 0:
+        raise ValueError("other_vehicles must be >= 0")
+    longi, lat = bool(act.get("longitudinal", True)), bool(act.get("lateral", True))
+    if not (longi or lat):
+        raise ValueError("Either longitudinal and/or lateral control must be enabled")
+    if act.get("dynamical", False):
+        raise NotImplementedError(f"dynamical=True (BicycleVehicle) on {env_id}")
+    # ContinuousAction checks the remaining keywords; it stands for the two-axis form the kernel reads
+    at = ContinuousAction(**dict(act, longitudinal=True, lateral=True))
+    action_size = 2 if longi and lat else 1
+    V = other + 1 if other > 0 else 1  # ego, front vehicle, integers(other_vehicles) < other_vehicles more
+    p = N.HwyNetParams()
+    p.n_vehicles = V
+    p.simulation_frequency, p.policy_frequency = int(cfg["simulation_frequency"]), int(cfg["policy_frequency"])
+    ts = np.array(act.get("target_speeds") or [0, 5, 10], dtype=np.float64)[:3]
+    p.n_target_speeds = int(ts.size)
+    for k, t in enumerate(ts):
+        p.target_speeds[k] = float(t)
+    # the kernel reads (throttle, steering) pairs; a missing axis is staged as 0 and maps to exactly 0 through the
+    # range (0, 0): 0 + ((0 - -1) * 0) / 2 = +0.0 in float32
+    p.action_type, p.act_clip, p.dynamical = 1, int(at.clip), 0
+    p.acc_lo, p.acc_hi = (float(at.acceleration_range[0]), float(at.acceleration_range[1])) if longi else (0.0, 0.0)
+    p.steer_lo, p.steer_hi = (float(at.steering_range[0]), float(at.steering_range[1])) if lat else (0.0, 0.0)
+    plugin, fused = select_network_observation(None, p, obs, ts, 2, fuse_ttc=False, fuse_grid=False,
+                                               feature_columns=True)
+    assert isinstance(plugin, (KinematicObservation, OccupancyGridObservation))
+    p.duration = float(cfg["duration"])
+    p.collision_reward = float(cfg["collision_reward"])
+    # IDMVehicle class constants (vehicle/behavior.py:21-46)
+    p.acc_max, p.comfort_acc_max, p.comfort_acc_min = 6.0, 3.0, -5.0
+    p.distance_wanted, p.time_wanted = 10.0, 1.5
+    p.politeness, p.lane_change_min_acc_gain = 0.0, 0.2
+    p.lane_change_max_braking_imposed, p.lane_change_delay = 2.0, 1.0
+    p.perception_distance = 200.0
+    p.connected_lanes = int(bool(cfg.get("neighbour_vehicles_connected_lanes", False)))
+    net = _host_network()
+    rp = N.HwyRacetrackParams()
+    rp.other_vehicles = other
+    rp.terminate_off_road = int(bool(cfg["terminate_off_road"]))
+    rp.lane_ab, rp.lane_bc = net.index[("a", "b", 0)], net.index[("b", "c", 0)]
+    rp.n_from_nodes = len(net._graph)
+    rp.lane_centering_cost = float(cfg["lane_centering_cost"])
+    rp.lane_centering_reward = float(cfg["lane_centering_reward"])
+    rp.action_reward = float(cfg["action_reward"])
+    rp.collision_reward = float(cfg["collision_reward"])
+    rp.on_road_reward = float(cfg.get("on_road_reward", 0))
+    return dict(params=p, race=rp, action_type=at, observation_type=plugin, fused=fused, lateral=lat,
+                action_size=action_size, V=V)
+
+
+class BatchedRacetrackEnv(BatchedNetworkEnv):
+    ENV_ID = "racetrack-v0"
+    # _rewards (:72-83), in the reference's order
+    REWARD_NAMES = ("lane_centering_reward", "action_reward", "collision_reward", "on_road_reward")
+    META_FLAGS = ("crashed", "has_impact", "check_collisions")
+    ROW_EXCLUDE = BatchedNetworkEnv.ROW_EXCLUDE | {"_pair_buf"}  # staging, rewritten by every step
+
+    def _make_network(self) -> NetworkTable:
+        return make_racetrack_network()
+
+    # ------------------------------------------------------------------ configuration
+    def define_spaces(self) -> None:
+        if self.reset_mode != "device":
+            raise NotImplementedError(f"{self.ENV_ID} resets on the device (hwy_racetrack_reset)")
+        spec = racetrack_params(self.config, self.ENV_ID)
+        self._params, self._race = spec["params"], spec["race"]
+        self.action_type, self.observation_type = spec["action_type"], spec["observation_type"]
+        self.lateral, self.action_size, self.V = spec["lateral"], spec["action_size"], spec["V"]
+        self._plugin_standalone = not spec["fused"]
+        self.single_observation_space = self.observation_type.space()
+        self.single_action_space = Box(-1.0, 1.0, shape=(self.action_size,), dtype=np.float32)
+        self.observation_space = batch_space(self.single_observation_space, self.num_envs)
+        self.action_space = batch_space(self.single_action_space, self.num_envs)
+        self.obs_shape = tuple(self.single_observation_space.shape)
+
+    def _allocate(self) -> None:
+        n = self.num_envs
+        self.net  # the lane table on the device (_graph_dev)
+        st = self._allocate_network_state(N.HWY_NET_GROUP)
+        self._count = torch.zeros(n, dtype=torch.int32, device=self.device)
+        st.count = self._count.data_ptr()
+        # the actions as passed [N, action_size]; with one control axis, the (throttle, steering) pairs the kernel reads
+        self._action_buf = torch.zeros(n, self.action_size, dtype=torch.float32, device=self.device)
+        self._pair_buf = None if self.action_size == 2 else torch.zeros(n, 2, dtype=torch.float32, device=self.device)
+
+    # ------------------------------------------------------------------ actions
+    def _stage_actions(self, actions) -> torch.Tensor:
+        act = super()._stage_actions(actions)
+        if self._pair_buf is not None:  # one control axis: the other stays 0
+            self._pair_buf[:, 1 if self.lateral else 0].copy_(act[:, 0])
+        return act
+
+    # ------------------------------------------------------------------ family kernels
+    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_racetrack_reset(
+                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
+                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
+
+    def _step_kernels(self, act) -> None:
+        pairs = act if self._pair_buf is None else self._pair_buf
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_racetrack_step(
+                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
+                pairs.data_ptr(), 0, self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
+                self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
+                self._stream()))
+
+    def road_substeps(self, n_substeps: int) -> None:
+        """`n_substeps` x (Road.act(); Road.step(1 / simulation_frequency)) of every env and nothing else; the plain
+        ego keeps the action of its last step (Vehicle.act(None), kinematics.py:119-128)."""
+        if not self._seeded:
+            raise RuntimeError("call reset() before road_substeps()")
+        if n_substeps < 0:
+            raise ValueError("n_substeps < 0")
+        if n_substeps == 0:
+            return
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_racetrack_step(
+                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
+                None, int(n_substeps), None, None, None, None, None, None, self._stream()))
+
+    def to_finite_mdp(self):
+        raise NotImplementedError(f"to_finite_mdp on {self.ENV_ID}: the finite MDP needs DiscreteMetaAction")
+
+    def get_available_actions(self):
+        raise NotImplementedError(f"get_available_actions on {self.ENV_ID}: ContinuousAction has no discrete actions")
+
+    # ------------------------------------------------------------------ state import / export
+    def _env_rows(self) -> dict:
+        rows = super()._env_rows()
+        rows["_count"] = self._count
+        return rows
+
+    def state_dict(self) -> dict:
+        """The per-vehicle fields [N, V]; `count` vehicles of each env are on the road.  The ego's target_speed /
+        timer hold its persisting (acceleration, steering) action."""
+        sd = super().state_dict()
+        del sd["rng"]  # per-env fields only; the streams are rng_words()
+        sd["count"] = self._count.cpu().numpy()
+        return sd
+
+    def load_state_dict(self, sd: dict, env_ids=None) -> None:
+        super().load_state_dict(sd, env_ids)
+        idx = slice(None) if env_ids is None else torch.from_numpy(np.asarray(env_ids, dtype=np.int64)).to(self.device)
+        self._count[idx] = torch.from_numpy(np.asarray(sd["count"], dtype=np.int32).reshape(-1)).to(self.device)
+        self._route_len[idx] = 0
+
+
+class BatchedConnectedLaneRacetrackEnv(BatchedRacetrackEnv):
+    """`racetrack-v1`: ConnectedLaneNeighboursMixin (envs/common/abstract.py:26-37)."""
+
+    ENV_ID = "racetrack-v1"

@@ -512,6 +512,33 @@ int hwy_roundabout_reset(const HwyNetParams *p, const HwyNetGraph *graph, const 
                          const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
                          float *obs, void *stream);
 
+/* RacetrackEnv (envs/racetrack_env.py:15-425; racetrack-v0, and racetrack-v1 with connected_lanes) on the 8-slot
+ * network state, which must carry s->count (the population: the ego, the front vehicle and the extra vehicles that
+ * survived the 20 m check).  The controlled vehicle is a plain Vehicle (HWY_KIND_VEHICLE) in slot 0 whose (target_speed,
+ * timer) pair holds its persisting action dict (acceleration, steering) (vehicle/kinematics.py:119-128); `action` is
+ * float32 [n_envs][2] = (throttle, steering) as passed, a missing control axis staged as 0 with the range (0, 0) in p. */
+typedef struct HwyRacetrackParams {
+    int32_t other_vehicles;      /* config["other_vehicles"], 0..HWY_NET_GROUP - 1 */
+    int32_t terminate_off_road;  /* config["terminate_off_road"] */
+    int32_t lane_ab, lane_bc;    /* table index of ("a","b",0) and ("b","c",0) */
+    int32_t n_from_nodes;        /* len(network.graph): random_lane_index draws among nodes 0 .. n-1 */
+    int32_t _pad;
+    double lane_centering_cost, lane_centering_reward, action_reward, collision_reward, on_road_reward;
+} HwyRacetrackParams;
+/* _make_vehicles (:374-425) for the envs selected by mask_a | mask_b (both NULL: all), drawing from rng[5*n_envs] in
+ * the reference's order; slots past the population are cleared.  obs != NULL: also their reset observation. */
+int hwy_racetrack_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyRacetrackParams *rp,
+                        const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
+                        float *obs, void *stream);
+/* n_substeps == 0: one RacetrackEnv.step of every env — the action, simulation_frequency / policy_frequency substeps,
+ * observation, reward (:66-83; s->reward_terms: lane_centering, action, collision, on_road), terminated (crashed, or
+ * off road with terminate_off_road), truncated (time >= duration).  n_substeps > 0: that many Road.act + Road.step
+ * with the persisting action and nothing else; action and the outputs are then not read or written (may be NULL). */
+int hwy_racetrack_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyRacetrackParams *rp,
+                       const HwyNetState *s, const float *action, int n_substeps, float *obs, double *reward,
+                       uint8_t *terminated, uint8_t *truncated, double *info_speed, uint8_t *info_crashed,
+                       void *stream);
+
 /* ====================================================================== observation plugins on ANY road family
  * The reference's observation_factory (envs/common/observation.py:772-794) builds any ObservationType on any env; these
  * entry points are that registry on the device: they read a state of either family through a HwyObsView (the highway
