@@ -316,6 +316,7 @@ EXPORTS = (
     "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
     "hwy_lane_keeping_reset", "hwy_lane_keeping_step", "hwy_racetrack_reset", "hwy_racetrack_step",
+    "hwy_debug_network_lanes", "hwy_debug_network_closest_lanes",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -323,6 +324,10 @@ MATH_OPS = {"sincos": (0, 1, 2), "idm_pow": (1, 2, 1), "exp_dlog": (2, 2, 1), "p
             "wrap_to_pi": (4, 1, 1), "not_zero": (5, 1, 1), "div_finite": (6, 2, 1), "dot2": (7, 4, 1),
             "norm2": (8, 2, 1), "beta_of_controlled": (9, 1, 2), "beta_of_angle": (10, 1, 2),
             "speed_to_index": (11, 2 + HWY_MAX_TARGET_SPEEDS, 1)}
+# hwy_debug_network_lanes ops and their result counts per input (HWY_LANES_IN operands each; include/hwyb200.h)
+HWY_LANES_IN = 5
+LANE_OPS = {"local": (0, 2), "position": (1, 2), "heading_at": (2, 1), "distance_with_heading": (3, 3), "on": (4, 1),
+            "maybe_on": (5, 1), "prunable": (6, 1), "prunable_scan": (7, HWY_NET_MAX_LANES)}
 # hwy_debug_pcg64 draw kinds
 PCG_OPS = {"next64": 0, "next32": 1, "next_double": 2, "uniform": 3, "normal": 4, "choice": 5, "pcg_at": 6}
 
@@ -369,6 +374,10 @@ def load():
     lib.hwy_intersection_step.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS] + [C.c_void_p] * 10
     lib.hwy_debug_network_neighbours.restype = C.c_int
     lib.hwy_debug_network_neighbours.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_debug_network_closest_lanes.restype = C.c_int
+    lib.hwy_debug_network_closest_lanes.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_debug_network_lanes.restype = C.c_int
+    lib.hwy_debug_network_lanes.argtypes = [C.POINTER(HwyNetGraph), C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
     lib.hwy_debug_rotated_rectangles_intersect.restype = C.c_int
     lib.hwy_debug_rotated_rectangles_intersect.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     lib.hwy_debug_math.restype = C.c_int

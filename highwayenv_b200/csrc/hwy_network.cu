@@ -1779,6 +1779,35 @@ debug_neighbours_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
         rear[slot] = rr;
     }
 }
+// Vehicle.on_state_update's closest-lane search alone, starting from the lanes in the state's meta words
+template <int G, bool REG>
+__global__ void __launch_bounds__(kBlockThreads)
+debug_closest_lanes_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
+                           const __grid_constant__ HwyNetState S, int32_t* __restrict__ lane,
+                           double* __restrict__ own_s, double* __restrict__ own_lat) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    GraphShared& g = *reinterpret_cast<GraphShared*>(smem_raw);
+    EnvStage<G, REG>* stages =
+        reinterpret_cast<EnvStage<G, REG>*>(smem_raw + ((sizeof(GraphShared) + 15) & ~size_t(15)));
+    stage_graph(g, graph);
+    constexpr int kEnvs = kBlockThreads / G;
+    const int sub = threadIdx.x / G, i = threadIdx.x % G;
+    const int env = blockIdx.x * kEnvs + sub;
+    const bool env_ok = env < S.n_envs;
+    const int e = env_ok ? env : S.n_envs - 1;
+    EnvStage<G, REG>& st = stages[sub];
+    Regs r;
+    load_env(P, g, S, st, e, i, r);
+    closest_lane_group(g, st, st.count, i, true);  // every thread of the block: the search has block barriers
+    if (env_ok) {
+        const size_t slot = (size_t)e * S.vp + i;
+        const bool on = i < st.count;
+        lane[slot] = on ? st.lane[i] : -1;
+        own_s[slot] = on ? st.own_s[i] : 0.0;
+        own_lat[slot] = on ? st.own_lat[i] : 0.0;
+    }
+}
+
 __global__ void debug_rectangles_kernel(const double* __restrict__ rects, int n, int32_t* __restrict__ out) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
@@ -2723,6 +2752,14 @@ int hwy_debug_network_neighbours(const HwyNetParams* p, const HwyNetGraph* graph
     if (!front || !rear) return fail("%s", "null pointer");
     return launch_groups([](auto t) { return hwynet::debug_neighbours_kernel<decltype(t)::G, decltype(t)::REG>; },
                          "debug_neighbours_kernel", s, (cudaStream_t)stream, *p, graph, *s, query_lane, front, rear);
+}
+
+int hwy_debug_network_closest_lanes(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s,
+                                    int32_t* lane, double* own_s, double* own_lat, void* stream) {
+    if (validate_net(p, graph, s)) return 1;
+    if (!lane || !own_s || !own_lat) return fail("%s", "null pointer");
+    return launch_groups([](auto t) { return hwynet::debug_closest_lanes_kernel<decltype(t)::G, decltype(t)::REG>; },
+                         "debug_closest_lanes_kernel", s, (cudaStream_t)stream, *p, graph, *s, lane, own_s, own_lat);
 }
 
 int hwy_debug_rotated_rectangles_intersect(const double* rects, int n, int32_t* out, void* stream) {

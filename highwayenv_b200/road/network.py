@@ -15,6 +15,7 @@ reference's network in tests/test_host_cpu.py).
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -22,6 +23,49 @@ import numpy as np
 from .. import _native as N
 
 LaneIndex = Tuple[str, str, int]
+
+
+def _two_sum(a, b):
+    """s + e == a + b exactly (Knuth)"""
+    s = a + b
+    bb = s - a
+    return s, (a - (s - bb)) + (b - bb)
+
+
+def _two_prod(a, b):
+    """h + l == a * b exactly (Dekker, Veltkamp splitting)"""
+    def split(x):
+        c = 134217729.0 * x  # 2^27 + 1
+        hi = c - (c - x)
+        return hi, x - hi
+
+    h = a * b
+    ah, al = split(a)
+    bh, bl = split(b)
+    return h, ((ah * bh - h) + ah * bl + al * bh) + al * bl
+
+
+def dot2(a0, a1, b0, b1):
+    """np.dot([a0, a1], [b0, b1]) element-wise: numpy's 2-vector dot is one fma, fma(a1, b1, a0 * b0) (pinned by
+    tests/test_rng_craft.py).  The exact value h + l + p is summed with error-free transformations; the few elements
+    whose rounding the fast sum cannot settle (within 2^-40 of a rounding boundary, or a power-of-two result) are
+    rounded by math.fsum."""
+    a0, a1, b0, b1 = (np.asarray(v, dtype=np.float64) for v in (a0, a1, b0, b1))
+    p = a0 * b0
+    h, l = _two_prod(a1, b1)
+    s, e = _two_sum(h, p)
+    t, f = _two_sum(e, l)
+    r, g = _two_sum(s, t)
+    z = g + f  # the exact value is r + g + f
+    with np.errstate(invalid="ignore", over="ignore"):
+        hard = ~(np.abs(z) < np.spacing(np.abs(r)) * (0.5 - 2.0 ** -40)) | (np.abs(np.frexp(r)[0]) == 0.5)
+    hard &= np.isfinite(h) & np.isfinite(p)
+    if hard.any():
+        r = np.array(r, dtype=np.float64, copy=True)
+        hb, lb, pb = np.broadcast_arrays(h, l, p)
+        for k in zip(*np.nonzero(hard)):
+            r[k] = math.fsum((float(hb[k]), float(lb[k]), float(pb[k])))
+    return r
 
 
 class NetworkTable:
@@ -239,11 +283,11 @@ class NetworkTable:
             dx, dy = x - L["cx"], y - L["cy"]
             phi = np.arctan2(dy, dx)
             phi = L["start_phase"] + (((phi - L["start_phase"]) + np.pi) % (2 * np.pi) - np.pi)
-            r = np.sqrt(dx * dx + dy * dy)
+            r = np.sqrt(dot2(dx, dy, dx, dy))  # np.linalg.norm
             return L["direction"] * (phi - L["start_phase"]) * L["radius"], L["direction"] * (L["radius"] - r)
         dx, dy = x - L["sx"], y - L["sy"]
-        lon = dx * L["dx"] + dy * L["dy"]
-        lat = dx * L["lx"] + dy * L["ly"]
+        lon = dot2(dx, dy, L["dx"], L["dy"])
+        lat = dot2(dx, dy, L["lx"], L["ly"])
         if L["type"] == N.LANE_SINE:
             lat = lat - L["amplitude"] * np.sin(L["pulsation"] * lon + L["phase"])
         return lon, lat

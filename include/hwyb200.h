@@ -393,6 +393,31 @@ int hwy_debug_network_neighbours(const HwyNetParams *p, const HwyNetGraph *graph
                                  const int32_t *query_lane, int32_t *front, int32_t *rear, void *stream);
 int hwy_debug_rotated_rectangles_intersect(const double *rects, int n, int32_t *out, void *stream);
 
+/* The lane functions of the network kernels (csrc/hwy_lanes.cuh) on n inputs, one thread each, on the lane table as
+ * the kernels stage it (the arcs' end points in sx, sy, ex, ey).  graph is a HOST pointer (1..HWY_NET_MAX_LANES
+ * lanes); in [n][HWY_LANES_IN] and out [n][k_out] are DEVICE doubles, in[0] the table index of the lane:
+ *   LOCAL lane, x, y -> s, lat (lane_local)               POSITION lane, s, lat -> x, y (lane_position)
+ *   HEADING_AT lane, s -> heading (lane_heading_at)
+ *   DISTANCE_WITH_HEADING lane, x, y, h -> d, s, lat (lane_distance_with_heading)
+ *   ON lane, x, y -> 1 / 0: lane_local, then lane_on(margin = 1)
+ *   MAYBE_ON lane, x, y -> 1 / 0: lane_maybe_on, the neighbour search's pre-test of ON
+ *   PRUNABLE lane, x, y, bd -> 1 / 0: closest_lane_prunable with a fresh circle cache
+ *   PRUNABLE_SCAN hint, x, y, bd -> [HWY_NET_MAX_LANES] closest_lane_prunable of every lane in table order with one
+ *                 circle cache carried across them, the hint skipped, as closest_lane_group scans (0 for the hint and
+ *                 past the table's end)
+ * An in[0] that is not a lane of the table gives NaN outputs. */
+#define HWY_LANES_IN 5
+enum {
+    HWY_LANES_LOCAL = 0, HWY_LANES_POSITION, HWY_LANES_HEADING_AT, HWY_LANES_DISTANCE_WITH_HEADING, HWY_LANES_ON,
+    HWY_LANES_MAYBE_ON, HWY_LANES_PRUNABLE, HWY_LANES_PRUNABLE_SCAN
+};
+int hwy_debug_network_lanes(const HwyNetGraph *graph, int op, const double *in, double *out, int n, void *stream);
+/* Vehicle.on_state_update's closest-lane search (closest_lane_group) of every vehicle of every env, the lane in each
+ * vehicle's meta word as the search's starting lane: lane [n_envs*vp] (-1 past the env's count), own_s / own_lat
+ * [n_envs*vp] its local coordinates on that lane.  graph is a DEVICE pointer, as for the step entry points. */
+int hwy_debug_network_closest_lanes(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetState *s,
+                                    int32_t *lane, double *own_s, double *own_lat, void *stream);
+
 /* The scalar device functions of the step kernels (csrc/hwy_math.cuh, csrc/hwy_device.cuh) on n inputs, one thread
  * each: in [n][k_in] and out [n][k_out] are DEVICE doubles; the operands of each op, in order, are
  *   SINCOS x -> sin, cos (m_sincos)          IDM_POW x, delta -> x ** delta     EXP_DLOG d, x -> exp(d log x)

@@ -20,7 +20,8 @@ def test_library_exports_every_declared_symbol():
     declared = set(re.findall(r"\b(hwy_[a-z_0-9]+)\s*\(", hdr))
     assert {"hwy_highway_step", "hwy_highway_reset", "hwy_highway_observe", "hwy_highway_substeps",
             "hwy_highway_slot_stride", "hwy_abi_version", "hwy_last_error", "hwy_launch_count",
-            "hwy_debug_math", "hwy_debug_pcg64"} <= declared
+            "hwy_debug_math", "hwy_debug_pcg64", "hwy_debug_network_lanes",
+            "hwy_debug_network_closest_lanes"} <= declared
     assert declared <= set(N.EXPORTS) | {"hwy_debug_phase_cycles"}
     for sym in declared:
         assert getattr(lib, sym) is not None, sym
@@ -66,7 +67,8 @@ def test_abi_validation_without_gpu():
 
 
 def test_test_entries_validate_their_arguments():
-    """hwy_debug_math / hwy_debug_pcg64 refuse bad ops, indices and pointers before touching the device."""
+    """hwy_debug_math / hwy_debug_pcg64 / hwy_debug_network_lanes / hwy_debug_network_closest_lanes refuse bad ops,
+    indices, pointers and lane tables before touching the device."""
     import ctypes as C
 
     from highwayenv_b200 import _native as N
@@ -93,6 +95,22 @@ def test_test_entries_validate_their_arguments():
     assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, 1, p, None, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
     assert pcg(N.PCG_OPS["normal"], 0, 0.0, 0.0, 1, p, p, None, 4, None) != 0 and b"null" in lib.hwy_last_error()
     assert pcg(N.PCG_OPS["next64"], 0, 0.0, 0.0, 1, p, p, p, -2, None) != 0 and b"n < 0" in lib.hwy_last_error()
+    lanes = lib.hwy_debug_network_lanes
+    g = N.HwyNetGraph()
+    g.n_lanes, g.n_nodes = 2, 2
+    assert lanes(C.byref(g), len(N.LANE_OPS), p, p, 4, None) != 0 and b"op" in lib.hwy_last_error()
+    assert lanes(C.byref(g), -1, p, p, 4, None) != 0 and b"op" in lib.hwy_last_error()
+    assert lanes(C.byref(g), 0, p, None, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert lanes(C.byref(g), 0, None, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert lanes(None, 0, p, p, 4, None) != 0 and b"null" in lib.hwy_last_error()
+    assert lanes(C.byref(g), 0, p, p, -1, None) != 0 and b"n < 0" in lib.hwy_last_error()
+    for n_lanes in (0, N.HWY_NET_MAX_LANES + 1):
+        g.n_lanes = n_lanes
+        assert lanes(C.byref(g), 0, p, p, 4, None) != 0 and b"n_lanes" in lib.hwy_last_error()
+    closest = lib.hwy_debug_network_closest_lanes
+    assert closest(None, None, None, p, p, p, None) != 0 and b"null" in lib.hwy_last_error()
+    np_, st = N.HwyNetParams(), N.HwyNetState()
+    assert closest(C.byref(np_), p, C.byref(st), p, p, p, None) != 0 and b"stride" in lib.hwy_last_error()
 
 
 def test_default_configs_match_reference_values():
