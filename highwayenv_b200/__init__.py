@@ -45,6 +45,11 @@ REGISTRY = {
     # a plain Vehicle steered round a two-lane track with IDM traffic; OccupancyGrid (presence, on_road)
     "racetrack-v0": "highwayenv_b200.envs.racetrack_env:BatchedRacetrackEnv",
     "racetrack-v1": "highwayenv_b200.envs.racetrack_env:BatchedConnectedLaneRacetrackEnv",
+    # the same task on the three-lane large track and on the oval of config["no_lanes"] lanes (2..4)
+    "racetrack-large-v0": "highwayenv_b200.envs.racetrack_env:BatchedRacetrackLargeEnv",
+    "racetrack-large-v1": "highwayenv_b200.envs.racetrack_env:BatchedConnectedLaneRacetrackLargeEnv",
+    "racetrack-oval-v0": "highwayenv_b200.envs.racetrack_env:BatchedRacetrackOvalEnv",
+    "racetrack-oval-v1": "highwayenv_b200.envs.racetrack_env:BatchedConnectedLaneRacetrackOvalEnv",
 }
 
 

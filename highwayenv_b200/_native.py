@@ -213,7 +213,7 @@ class HwyRoundaboutSpawn(C.Structure):
 
 class HwyRacetrackParams(C.Structure):
     _fields_ = [("other_vehicles", C.c_int32), ("terminate_off_road", C.c_int32), ("lane_ab", C.c_int32),
-                ("lane_bc", C.c_int32), ("n_from_nodes", C.c_int32), ("_pad", C.c_int32),
+                ("lane_bc", C.c_int32), ("n_from_nodes", C.c_int32), ("ego_lanes", C.c_int32),
                 ("lane_centering_cost", C.c_double), ("lane_centering_reward", C.c_double),
                 ("action_reward", C.c_double), ("collision_reward", C.c_double), ("on_road_reward", C.c_double)]
 

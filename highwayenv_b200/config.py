@@ -400,3 +400,17 @@ def racetrack_default_config() -> dict:
 
 DEFAULTS["racetrack-v0"] = racetrack_default_config
 DEFAULTS["racetrack-v1"] = _connected(racetrack_default_config)
+# RacetrackEnvLarge keeps RacetrackEnv.default_config
+DEFAULTS["racetrack-large-v0"] = racetrack_default_config
+DEFAULTS["racetrack-large-v1"] = _connected(racetrack_default_config)
+
+
+def racetrack_oval_default_config() -> dict:
+    """RacetrackEnvOval.default_config (highway_env/envs/racetrack_env.py:894-934): RacetrackEnv's and the oval's keys."""
+    config = racetrack_default_config()
+    update_config(config, {"length": 100, "no_lanes": 3, "block_lane": False, "force_decision": False})
+    return config
+
+
+DEFAULTS["racetrack-oval-v0"] = racetrack_oval_default_config
+DEFAULTS["racetrack-oval-v1"] = _connected(racetrack_oval_default_config)

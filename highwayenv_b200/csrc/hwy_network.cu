@@ -2294,11 +2294,12 @@ two_way_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* 
 }
 
 // ------------------------------------------------------------------ racetrack-v0 / v1 (envs/racetrack_env.py)
-// RacetrackEnv._make_vehicles (:374-425), one env per thread: the plain Vehicle on ("a","b",integers(2)) at
+// RacetrackEnv._make_vehicles (:374-425), one env per thread: the plain Vehicle on ("a","b",integers(ego_lanes)) at
 // uniform(20, 50) and the lane's speed limit; with other_vehicles > 0 the IDMVehicle on ("b","c", the ego's lane id) at
 // uniform(0, length of ("b","c",0)), speed 6 + uniform(0, 3); then integers(other_vehicles) attempts on
 // random_lane_index, each dropped when it lands closer than 20 m to a vehicle already placed.  No randomize_behavior:
-// DELTA stays 4.  The slots past the population are cleared.
+// DELTA stays 4.  The slots past the population are cleared.  ego_lanes is 2 on racetrack-v0 / v1 and on the large track
+// (RacetrackEnvLarge inherits this _make_vehicles) and no_lanes on the oval (RacetrackEnvOval._make_vehicles, :1340-1392).
 __global__ void __launch_bounds__(128)
 racetrack_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
                        const __grid_constant__ HwyRacetrackParams RP, const __grid_constant__ HwyNetState S,
@@ -2326,7 +2327,7 @@ racetrack_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph
         ys[n] = py;
         ++n;
     };
-    const int ego_id = g.choice(2);
+    const int ego_id = g.choice(RP.ego_lanes);
     const double ego_lon = g.uniform(20.0, 50.0);
     place(RP.lane_ab + ego_id, ego_lon, graph->lanes[RP.lane_ab + ego_id].speed_limit, HWY_KIND_VEHICLE, false);
     if (RP.other_vehicles > 0) {
@@ -2649,7 +2650,10 @@ int validate_racetrack(const HwyNetParams* p, const HwyRacetrackParams* rp, cons
     if (s->vp != HWY_NET_GROUP || !s->count) return fail("%s", "racetrack: slot stride 8 and the count buffer");
     if (rp->other_vehicles < 0 || rp->other_vehicles > HWY_NET_GROUP - 1)
         return fail("%s", "racetrack: other_vehicles out of range (0..7)");
-    if (rp->lane_ab < 0 || rp->lane_ab + 1 >= HWY_NET_MAX_LANES || rp->lane_bc < 0 || rp->lane_bc + 1 >= HWY_NET_MAX_LANES)
+    if (rp->ego_lanes < 1 || rp->ego_lanes > HWY_NET_MAX_LANES) return fail("%s", "racetrack: ego_lanes out of range");
+    // the ego's lane_ab + k and the front vehicle's lane_bc + k, k < ego_lanes, stay inside the lane table
+    if (rp->lane_ab < 0 || rp->lane_ab + rp->ego_lanes > HWY_NET_MAX_LANES || rp->lane_bc < 0 ||
+        rp->lane_bc + rp->ego_lanes > HWY_NET_MAX_LANES)
         return fail("%s", "racetrack: lane index out of range");
     if (rp->n_from_nodes < 1 || rp->n_from_nodes > HWY_NET_MAX_NODES) return fail("%s", "racetrack: n_from_nodes out of range");
     if (p->action_type != 1 || p->dynamical) return fail("%s", "racetrack: ContinuousAction with a plain Vehicle only");

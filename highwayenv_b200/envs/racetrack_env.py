@@ -1,4 +1,4 @@
-"""Batched racetrack-v0 / racetrack-v1 on the H100 backend.
+"""Batched racetrack-v0 / racetrack-v1, racetrack-large-v0 / v1 and racetrack-oval-v0 / v1 on the H100 backend.
 
 Host-side mirror of the reference's ``RacetrackEnv`` (highway_env/envs/racetrack_env.py:15-425): a closed two-lane
 track of 9 roads (straight and circular, width 5, speed limit 10), one controlled plain ``Vehicle`` steered through
@@ -12,6 +12,9 @@ with a plain ego, then the racetrack reward (:66-83), termination (crash, or off
 truncation at ``duration``.  Resets run in ``hwy_racetrack_reset`` from each env's numpy stream, in the reference's
 draw order (:374-425).  The plain Vehicle's action dict persists between steps (kinematics.py:119-128): the state
 keeps it in the ego's (target_speed, timer) pair as (acceleration, steering), which ``road_substeps`` replays.
+
+The large track (``RacetrackEnvLarge``, 9 roads x 3 lanes) and the oval (``RacetrackEnvOval``, 8 roads x ``no_lanes``)
+run on the same kernels with their own lane tables; only the ego's lane draw differs (``HwyRacetrackParams.ego_lanes``).
 """
 from __future__ import annotations
 
@@ -68,19 +71,154 @@ def make_racetrack_network() -> NetworkTable:
     return net
 
 
-_HOST_NET = None
+def make_racetrack_large_network(speed_limit: float = 10.0) -> NetworkTable:
+    """RacetrackEnvLarge._make_road (racetrack_env.py:439-875): 9 roads x 3 lanes, width 5, every lane at
+    config["speed_limit"], lanes in the reference's insertion order.  The end points of the slants and the arc centres
+    are computed with the reference's float64 expressions, in its order.  Some arcs end at different angles on their
+    lanes (136 / 137 / 137 deg, 202 / 205 / 205 deg, 210-88 / 210-90 / 212-88 deg); they are copied as they are."""
+    net = NetworkTable()
+    d = np.deg2rad
+    w, w2 = 5, 10
+
+    def straight(f, t, start, end, lt):
+        net.add_straight(f, t, start, end, width=w, speed_limit=speed_limit)
+        net._graph[f][t][-1]["line_types"] = list(lt)
+
+    def arc(f, t, center, radius, a0, a1, lt, clockwise=False):
+        net.add_circular(f, t, center, radius, d(a0), d(a1), clockwise=clockwise, width=w, speed_limit=speed_limit)
+        net._graph[f][t][-1]["line_types"] = list(lt)
+
+    straight("a", "b", [42, 0], [200, 0], (_C, _S))
+    straight("a", "b", [42, w], [200, w], (_S, _S))
+    straight("a", "b", [42, w2], [200, w2], (_N, _C))
+    arc("b", "c", [200, -20], 20, 90, -1, (_C, _N))
+    arc("b", "c", [200, -20], 20 + w, 90, -1, (_S, _S))
+    arc("b", "c", [200, -20], 20 + w2, 90, -1, (_N, _C))
+    straight("c", "d", [220, -20], [220, -60 + -1.0], (_C, _N))
+    straight("c", "d", [220 + w, -20], [220 + w, -60 + -1.0], (_S, _S))
+    straight("c", "d", [220 + w2, -20], [220 + w2, -60 + -1.0], (_N, _C))
+    arc("d", "e", [205, -60], 15, 0, -181, (_C, _N))
+    arc("d", "e", [205, -60], 15 + w, 0, -181, (_S, _S))
+    arc("d", "e", [205, -60], 15 + w2, 0, -181, (_N, _C))
+    arc("e", "f", [170, -60], 15 + 5, 0, 136, (_C, _N), clockwise=True)
+    arc("e", "f", [170, -60], 15, 0, 137, (_S, _S), clockwise=True)
+    arc("e", "f", [170, -60], 15 - w, 0, 137, (_N, _C), clockwise=True)
+    extend = np.array([-30, -30])
+    start6, end6 = np.array([155.7, -45.7]), np.array([135.7, -65.7]) + extend
+    start6_2, end6_2 = np.array([159.3934, -49.2]), np.array([139.3934, -69.2]) + extend
+    start6_3 = np.array([start6[0] + 2 * (start6_2[0] - start6[0]), start6[1] + 2 * (start6_2[1] - start6[1])])
+    end6_3 = np.array([end6[0] + 2 * (end6_2[0] - end6[0]), end6[1] + 2 * (end6_2[1] - end6[1])])
+    straight("f", "g", start6, end6, (_C, _N))
+    straight("f", "g", start6_2, end6_2, (_S, _S))
+    straight("f", "g", start6_3, end6_3, (_N, _C))
+    center7, r7, theta7, theta7_end = np.array([118.1, -48.1]) + extend, 25, 317, 205
+    arc("g", "h", center7, r7, theta7, theta7_end - 3, (_C, _N))
+    arc("g", "h", center7, r7 + 5, theta7, theta7_end, (_S, _S))
+    arc("g", "h", center7, r7 + w2, theta7, theta7_end, (_N, _C))
+    r9, rad = 15, d(30)
+    starts8 = [np.array([center7[0] + r * np.cos(d(theta7_end)), center7[1] + r * np.sin(d(theta7_end))])
+               for r in (r7, r7 + w, r7 + w2)]
+    ends8 = [np.array([42 - r * np.cos(rad), -r9 - r * np.sin(rad)]) for r in (r9, r9 + w, r9 + w2)]
+    straight("h", "i", starts8[0], ends8[0], (_C, _N))
+    straight("h", "i", starts8[1], ends8[1], (_S, _S))
+    straight("h", "i", starts8[2], ends8[2], (_N, _C))
+    center9 = np.array([42, -r9])
+    arc("i", "a", center9, r9, 210, 88, (_C, _N))
+    arc("i", "a", center9, r9 + w, 210, 90, (_S, _S))
+    arc("i", "a", center9, r9 + w2, 212, 88, (_N, _C))
+    net.finalize()
+    return net
 
 
-def _host_network() -> NetworkTable:
-    global _HOST_NET
-    if _HOST_NET is None:
-        _HOST_NET = make_racetrack_network()
-    return _HOST_NET
+OVAL_MAX_LANES = 4  # 8 roads x 4 lanes fill the 32-lane table
+
+
+def make_racetrack_oval_network(length: float = 100, no_lanes: int = 3) -> NetworkTable:
+    """RacetrackEnvOval._make_road (racetrack_env.py:936-1337) for a given `length` of the horizontal straights and
+    `no_lanes` lanes per road: 8 roads, width 5, speed limit 10, lanes in the reference's insertion order (the inner
+    lane, the middle lanes outwards, the outer lane).  The roadblock obstacles are not part of the network."""
+    if not 2 <= no_lanes <= OVAL_MAX_LANES:
+        raise ValueError(f"no_lanes must be in 2..{OVAL_MAX_LANES}")
+    net = NetworkTable()
+    d = np.deg2rad
+    n = no_lanes
+
+    def lane_types(inner, middle):
+        return [inner] + [middle] * (n - 2) + [(_S, _C)]  # the inner lane, the middle lanes, the outer lane
+
+    def straights(f, t, ends, lts):
+        for (start, end), lt in zip(ends, lts):
+            net.add_straight(f, t, start, end, width=5, speed_limit=10.0)
+            net._graph[f][t][-1]["line_types"] = list(lt)
+
+    def arcs(f, t, center, radius, a0, a1, lts):
+        for i, lt in enumerate(lts):
+            net.add_circular(f, t, center, radius + i * 5, d(a0), d(a1), clockwise=False, width=5, speed_limit=10.0)
+            net._graph[f][t][-1]["line_types"] = list(lt)
+
+    turn, side = lane_types((_C, _N), (_S, _N)), range(n)
+    straights("a", "b", [([0, i * 5], [length + 1, i * 5]) for i in side], lane_types((_C, _S), (_S, _N)))
+    arcs("b", "c", [length, -20], 20, 90, 0, turn)
+    straights("c", "d", [([length + 20 + i * 5, -20], [length + 20 + i * 5, -50]) for i in side], turn)
+    arcs("d", "e", [length + 5, -50], 15, 0, -90, turn)
+    straights("e", "f", [([length + 5, -(65 + i * 5)], [-5, -(65 + i * 5)]) for i in side], turn)
+    arcs("f", "g", [-5, -50], 15, -90, -180, turn)
+    straights("g", "h", [([-20 - i * 5, -50], [-20 - i * 5, -20]) for i in side], turn)
+    arcs("h", "a", [0, -20], 20, 180, 90, lane_types((_C, _N), (_S, _C)))  # its middle lanes: (STRIPED, CONTINUOUS)
+    net.finalize()
+    return net
+
+
+_HOST_NETS: dict = {}
+
+
+def track_network(env_id: str, cfg: dict) -> NetworkTable:
+    """The lane table of `env_id` under `cfg` (cached per track): racetrack-v0 / v1, the large track at
+    config["speed_limit"], or the oval of config["length"] and config["no_lanes"] (already checked)."""
+    base = env_id.rsplit("-", 1)[0]
+    if base == "racetrack-large":
+        key = (base, float(cfg["speed_limit"]))
+    elif base == "racetrack-oval":
+        key = (base, cfg["length"], int(cfg["no_lanes"]))
+    else:
+        key = ("racetrack",)
+    if key not in _HOST_NETS:
+        if key[0] == "racetrack-large":
+            _HOST_NETS[key] = make_racetrack_large_network(key[1])
+        elif key[0] == "racetrack-oval":
+            _HOST_NETS[key] = make_racetrack_oval_network(key[1], key[2])
+        else:
+            _HOST_NETS[key] = make_racetrack_network()
+    return _HOST_NETS[key]
+
+
+def _check_oval(cfg: dict, env_id: str) -> None:
+    """The oval's own keys (RacetrackEnvOval.default_config, :894-934) that the accelerated path does not run."""
+    length, no_lanes = cfg["length"], cfg["no_lanes"]
+    if no_lanes == 0 or length == 0:
+        raise NotImplementedError(f"random length / no_lanes (0) on {env_id}: the reference draws them from an "
+                                  "unseeded np.random.default_rng(), which no seed reproduces")
+    if isinstance(no_lanes, bool) or int(no_lanes) != no_lanes or no_lanes < 0:
+        raise ValueError("no_lanes must be a non-negative integer")
+    if no_lanes > OVAL_MAX_LANES:
+        raise NotImplementedError(f"no_lanes > {OVAL_MAX_LANES} on {env_id}: 8 roads x {no_lanes} lanes exceed the "
+                                  f"{N.HWY_NET_MAX_LANES}-lane table")
+    if no_lanes == 1:
+        raise ValueError("no_lanes 1: the reference builds the inner and the outer lane on the same line")
+    if isinstance(length, bool) or not np.isfinite(float(length)) or length < 0:
+        raise ValueError("length must be a positive number")
+    for key in ("block_lane", "force_decision"):
+        if cfg.get(key, False):
+            raise NotImplementedError(f"{key}=True on {env_id}: its Obstacles do not fit the 8-slot state")
 
 
 def racetrack_params(cfg: dict, env_id: str = "racetrack-v0") -> dict:
     """The kernel parameters of a racetrack config (HwyNetParams, HwyRacetrackParams) and its action / observation
-    plugins; raises for what the accelerated path does not run, before anything touches the device."""
+    plugins; raises for what the accelerated path does not run, before anything touches the device.  `env_id` picks
+    the track: racetrack-v0 / v1, racetrack-large-v0 / v1 or racetrack-oval-v0 / v1."""
+    oval = env_id.startswith("racetrack-oval")
+    if oval:
+        _check_oval(cfg, env_id)
     act, obs = cfg["action"], cfg["observation"]
     if act["type"] != "ContinuousAction":
         raise NotImplementedError(f"action type {act['type']!r} on {env_id} (ContinuousAction only)")
@@ -115,7 +253,11 @@ def racetrack_params(cfg: dict, env_id: str = "racetrack-v0") -> dict:
     p.action_type, p.act_clip, p.dynamical = 1, int(at.clip), 0
     p.acc_lo, p.acc_hi = (float(at.acceleration_range[0]), float(at.acceleration_range[1])) if longi else (0.0, 0.0)
     p.steer_lo, p.steer_hi = (float(at.steering_range[0]), float(at.steering_range[1])) if lat else (0.0, 0.0)
-    plugin, fused = select_network_observation(None, p, obs, ts, 2, fuse_ttc=False, fuse_grid=False,
+    net = track_network(env_id, cfg)
+    # Kinematics' default y range spans all_side_lanes of the ego's spawn road ("a","b"): 2 lanes on racetrack-v0,
+    # 3 on the large track, no_lanes on the oval
+    ab_lanes = net.lanes[net.index[("a", "b", 0)]]["road_count"]
+    plugin, fused = select_network_observation(None, p, obs, ts, ab_lanes, fuse_ttc=False, fuse_grid=False,
                                                feature_columns=True)
     assert isinstance(plugin, (KinematicObservation, OccupancyGridObservation))
     p.duration = float(cfg["duration"])
@@ -127,19 +269,24 @@ def racetrack_params(cfg: dict, env_id: str = "racetrack-v0") -> dict:
     p.lane_change_max_braking_imposed, p.lane_change_delay = 2.0, 1.0
     p.perception_distance = 200.0
     p.connected_lanes = int(bool(cfg.get("neighbour_vehicles_connected_lanes", False)))
-    net = _host_network()
     rp = N.HwyRacetrackParams()
     rp.other_vehicles = other
     rp.terminate_off_road = int(bool(cfg["terminate_off_road"]))
     rp.lane_ab, rp.lane_bc = net.index[("a", "b", 0)], net.index[("b", "c", 0)]
     rp.n_from_nodes = len(net._graph)
+    # the ego's lane draw: integers(2) in RacetrackEnv._make_vehicles (also the large track's), integers(no_lanes) in
+    # the oval's; the front vehicle takes the same lane id on ("b","c")
+    rp.ego_lanes = int(cfg["no_lanes"]) if oval else 2
+    # hwy_racetrack_reset cannot read the device table; the lane ids it draws must exist on both roads
+    if rp.ego_lanes > min(net.lanes[rp.lane_ab]["road_count"], net.lanes[rp.lane_bc]["road_count"]):
+        raise ValueError(f"ego_lanes {rp.ego_lanes} exceeds the lanes of ('a','b') or ('b','c') on {env_id}")
     rp.lane_centering_cost = float(cfg["lane_centering_cost"])
     rp.lane_centering_reward = float(cfg["lane_centering_reward"])
     rp.action_reward = float(cfg["action_reward"])
     rp.collision_reward = float(cfg["collision_reward"])
     rp.on_road_reward = float(cfg.get("on_road_reward", 0))
     return dict(params=p, race=rp, action_type=at, observation_type=plugin, fused=fused, lateral=lat,
-                action_size=action_size, V=V)
+                action_size=action_size, V=V, net=net)
 
 
 class BatchedRacetrackEnv(BatchedNetworkEnv):
@@ -150,13 +297,18 @@ class BatchedRacetrackEnv(BatchedNetworkEnv):
     ROW_EXCLUDE = BatchedNetworkEnv.ROW_EXCLUDE | {"_pair_buf"}  # staging, rewritten by every step
 
     def _make_network(self) -> NetworkTable:
-        return make_racetrack_network()
+        return self._track
 
     # ------------------------------------------------------------------ configuration
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
             raise NotImplementedError(f"{self.ENV_ID} resets on the device (hwy_racetrack_reset)")
         spec = racetrack_params(self.config, self.ENV_ID)
+        # the lane table follows the config (the oval's length / no_lanes, the large track's speed_limit): after
+        # reset(options={"config": ...}) picks another track, `net` rebuilds the table and its device copy
+        if self._net is not spec["net"]:
+            self._net = None
+        self._track = spec["net"]
         self._params, self._race = spec["params"], spec["race"]
         self.action_type, self.observation_type = spec["action_type"], spec["observation_type"]
         self.lateral, self.action_size, self.V = spec["lateral"], spec["action_size"], spec["V"]
@@ -220,6 +372,14 @@ class BatchedRacetrackEnv(BatchedNetworkEnv):
     def get_available_actions(self):
         raise NotImplementedError(f"get_available_actions on {self.ENV_ID}: ContinuousAction has no discrete actions")
 
+    def copy_envs(self, dst_ids, src_ids, source=None) -> None:
+        """BatchedVectorEnv.copy_envs; two envs of one class may still run different tracks (the oval's length /
+        no_lanes, the large track's speed_limit), and a state only means something on its own lane table."""
+        if source is not None and type(source) is type(self) and source._track is not self._track:
+            raise ValueError(f"copy_envs between {self.ENV_ID} envs on different tracks (length, no_lanes or "
+                             "speed_limit)")
+        super().copy_envs(dst_ids, src_ids, source)
+
     # ------------------------------------------------------------------ state import / export
     def _env_rows(self) -> dict:
         rows = super()._env_rows()
@@ -245,3 +405,31 @@ class BatchedConnectedLaneRacetrackEnv(BatchedRacetrackEnv):
     """`racetrack-v1`: ConnectedLaneNeighboursMixin (envs/common/abstract.py:26-37)."""
 
     ENV_ID = "racetrack-v1"
+
+
+class BatchedRacetrackLargeEnv(BatchedRacetrackEnv):
+    """`racetrack-large-v0`: RacetrackEnvLarge (racetrack_env.py:432-875), the three-lane track of 27 lanes with
+    RacetrackEnv's config, rules and _make_vehicles (the ego on ("a","b",integers(2)))."""
+
+    ENV_ID = "racetrack-large-v0"
+
+
+class BatchedConnectedLaneRacetrackLargeEnv(BatchedRacetrackLargeEnv):
+    """`racetrack-large-v1`: ConnectedLaneNeighboursMixin over the large track."""
+
+    ENV_ID = "racetrack-large-v1"
+
+
+class BatchedRacetrackOvalEnv(BatchedRacetrackEnv):
+    """`racetrack-oval-v0`: RacetrackEnvOval (racetrack_env.py:882-1392), an oval of 8 roads x config["no_lanes"] lanes
+    (2..4) with horizontal straights of config["length"]; the ego on ("a","b",integers(no_lanes)).  Random length /
+    no_lanes (0) and the block_lane / force_decision obstacles raise."""
+
+    ENV_ID = "racetrack-oval-v0"
+
+
+
+class BatchedConnectedLaneRacetrackOvalEnv(BatchedRacetrackOvalEnv):
+    """`racetrack-oval-v1`: ConnectedLaneNeighboursMixin over the oval."""
+
+    ENV_ID = "racetrack-oval-v1"

@@ -537,8 +537,8 @@ int hwy_roundabout_reset(const HwyNetParams *p, const HwyNetGraph *graph, const 
                          const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
                          float *obs, void *stream);
 
-/* RacetrackEnv (envs/racetrack_env.py:15-425; racetrack-v0, and racetrack-v1 with connected_lanes) on the 8-slot
- * network state, which must carry s->count (the population: the ego, the front vehicle and the extra vehicles that
+/* RacetrackEnv (envs/racetrack_env.py:15-425; racetrack-v0, and racetrack-v1 with connected_lanes) and its large
+ * (RacetrackEnvLarge, :432-880) and oval (RacetrackEnvOval, :882-1396) tracks on the 8-slot network state, which must carry s->count (the population: the ego, the front vehicle and the extra vehicles that
  * survived the 20 m check).  The controlled vehicle is a plain Vehicle (HWY_KIND_VEHICLE) in slot 0 whose (target_speed,
  * timer) pair holds its persisting action dict (acceleration, steering) (vehicle/kinematics.py:119-128); `action` is
  * float32 [n_envs][2] = (throttle, steering) as passed, a missing control axis staged as 0 with the range (0, 0) in p. */
@@ -547,7 +547,8 @@ typedef struct HwyRacetrackParams {
     int32_t terminate_off_road;  /* config["terminate_off_road"] */
     int32_t lane_ab, lane_bc;    /* table index of ("a","b",0) and ("b","c",0) */
     int32_t n_from_nodes;        /* len(network.graph): random_lane_index draws among nodes 0 .. n-1 */
-    int32_t _pad;
+    int32_t ego_lanes;           /* the ego's lane draw integers(ego_lanes): 2 (racetrack, large), no_lanes (oval);
+                                  * at most the lane count of ("a","b") and of ("b","c"), which the caller checks */
     double lane_centering_cost, lane_centering_reward, action_reward, collision_reward, on_road_reward;
 } HwyRacetrackParams;
 /* _make_vehicles (:374-425) for the envs selected by mask_a | mask_b (both NULL: all), drawing from rng[5*n_envs] in

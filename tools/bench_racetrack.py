@@ -1,18 +1,21 @@
-"""racetrack-v0 throughput on one GPU, and the reference's per-core rate on a CPU host.
+"""racetrack throughput on one GPU, and the reference's per-core rate on a CPU host.
 
-    python tools/bench_racetrack.py [--envs 65536 1048576] [--steps 200] [--warmup 50] [--runs 5] [--out r.json]
+    python tools/bench_racetrack.py [--env-id racetrack-v0] [--envs 65536 1048576] [--steps 200] [--warmup 50]
+                                    [--runs 5] [--out r.json]
     python tools/bench_racetrack.py --reference [--seconds 20]     # CPU host with the reference checkout
 
-GPU mode, per env count, SameStep autoreset, the default configuration (one front vehicle, the 2 x 12 x 12
+GPU mode, per env count, on --env-id (racetrack-v0 by default; racetrack-large-v0 / v1 and racetrack-oval-v0 / v1
+run the same kernels on their own lane tables), SameStep autoreset, the default configuration (one front vehicle, the 2 x 12 x 12
 OccupancyGrid aligned with the vehicle), seeded uniform steering in [-1, 1] staged on the device beforehand (a pool of
 16 tensors, cycled):
   * env-steps/s of `env.step` over --steps steps between two CUDA events on the stream, after --warmup steps; the
     median (min, max) of --runs windows.  The windows span the autoresets, which run inside `env.step`;
   * the step kernel alone: the same windows summed over CUDA events around each launch (`env._kernel_events`);
-  * the standalone grid kernel alone (`hwy_observe_grid`, which samples the on_road layer on all 18 lanes for every
-    cell of every env): --steps launches on the current state between two CUDA events, and its time as a share of
+  * the standalone grid kernel alone (`hwy_observe_grid`, which samples the on_road layer on every lane of the table
+    for every cell of every env: 18 on racetrack-v0, 27 on the large track, 24 on the default oval): --steps launches on the current state between two CUDA events, and its time as a share of
     the `env.step` window.
-The card's name and power limit are read in the same run.  Reference mode times `RacetrackEnv.step` of the unmodified
+The card's name and power limit are read in the same run; with an --env-id other than racetrack-v0 the JSON line
+also names it.  Reference mode times `RacetrackEnv.step` of the unmodified
 reference on one core (with `reset()` after each terminated episode), the per-core rate a CPU vector env gets.
 """
 from __future__ import annotations
@@ -29,12 +32,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def bench_gpu(n: int, steps: int, warmup: int, runs: int) -> dict:
+def bench_gpu(n: int, steps: int, warmup: int, runs: int, env_id: str = "racetrack-v0") -> dict:
     import torch
 
     import highwayenv_b200 as hb
 
-    env = hb.make("racetrack-v0", num_envs=n, autoreset_mode="SameStep")
+    env = hb.make(env_id, num_envs=n, autoreset_mode="SameStep")
     env.reset(seed=0)
     gen = torch.Generator(device=env.device).manual_seed(0)
     pool = [torch.rand(n, 1, device=env.device, generator=gen) * 2 - 1 for _ in range(16)]
@@ -91,6 +94,7 @@ def bench_reference(seconds: float) -> dict:
 
 def main() -> None:
     ap = argparse.ArgumentParser()
+    ap.add_argument("--env-id", default="racetrack-v0", help="GPU mode: the racetrack id to measure")
     ap.add_argument("--envs", type=int, nargs="+", default=[65536, 1048576])
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=50)
@@ -111,7 +115,10 @@ def main() -> None:
         sys.path.insert(0, os.path.join(ROOT, "tools"))
         from bench_opd import gpu_info
 
-        res = {"gpu": gpu_info(), "results": [bench_gpu(n, args.steps, args.warmup, args.runs) for n in args.envs]}
+        res = {"gpu": gpu_info(),
+               "results": [bench_gpu(n, args.steps, args.warmup, args.runs, args.env_id) for n in args.envs]}
+        if args.env_id != "racetrack-v0":
+            res["env_id"] = args.env_id
     line = json.dumps(res)
     print(line)
     if args.out:
