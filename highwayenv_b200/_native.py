@@ -56,7 +56,8 @@ class HwyHighwayParams(C.Structure):
             "lane_change_min_acc_gain", "lane_change_max_braking_imposed", "lane_change_delay",
             "delta_lo", "delta_hi", "perception_distance")]
         + [("lanes", HwyStraightLane * HWY_MAX_LANES)]
-        + [("obs_n_features", C.c_int32), ("_pad_obs", C.c_int32),
+        + [("obs_n_features", C.c_int32), ("n_agents", C.c_int16), ("multi_action", C.c_uint8),
+           ("multi_obs", C.c_uint8),
            ("obs_feature", C.c_int32 * HWY_MAX_OBS_FEATURES), ("obs_feature_ranged", C.c_int32 * HWY_MAX_OBS_FEATURES),
            ("obs_feature_lo", C.c_double * HWY_MAX_OBS_FEATURES), ("obs_feature_hi", C.c_double * HWY_MAX_OBS_FEATURES)]
     )

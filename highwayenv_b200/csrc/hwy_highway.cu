@@ -366,17 +366,18 @@ __device__ __noinline__ void kinematics_row_features(const HwyHighwayParams& P, 
 }
 
 // DENSE (dense step kernels): threads i >= V own no vehicle and store nothing; the V threads pad the missing rows.
+// `o`: the observer's slot (observer_vehicle; the multi-agent kernels observe from every controlled vehicle).
 template <int TPE, bool DENSE = false>
 __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, const Frame<TPE>& F,
                                                    double* key_scratch, int i, double heading,
                                                    float* __restrict__ obs_env,
-                                                   float* __restrict__ obs_env2 = nullptr) {
+                                                   float* __restrict__ obs_env2 = nullptr, const int o = 0) {
     const int V = P.n_vehicles, K = P.obs_vehicles_count;
-    const HwyStraightLane& Le = P.lanes[F.lane[0]];
-    const double ex = F.x[0], ey = F.y[0];
-    const double evx = F.v[0] * F.c[0], evy = F.v[0] * F.s[0];
+    const HwyStraightLane& Le = P.lanes[F.lane[o]];
+    const double ex = F.x[o], ey = F.y[o];
+    const double evx = F.v[o] * F.c[o], evy = F.v[o] * F.s[o];
     double key = INFINITY;
-    if (i > 0 && i < V) {
+    if ((o == 0 ? i > 0 : i != o) && i < V) {  // (a dense kernel's i is not known to be >= 0)
         bool ok = norm2(F.x[i] - ex, F.y[i] - ey) < P.perception_distance;
         double d = lane_s(Le, F.x[i], F.y[i]) - lane_s(Le, ex, ey);
         ok = ok && (P.obs_see_behind || -2 * kVehLength < d);
@@ -386,7 +387,7 @@ __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, co
     env_sync<TPE>();
     // stable rank among the valid candidates (python sorted() on |lane_distance_to|)
     int rank = 0, n_valid = 0;
-    for (int u = 1; u < V; ++u) {
+    for (int u = o == 0 ? 1 : 0; u < V; ++u) {  // (the observer's key is INFINITY)
         double ku = key_scratch[u];
         n_valid += ku < INFINITY;
         rank += (ku < key) || (ku == key && u < i);
@@ -398,7 +399,7 @@ __device__ __forceinline__ void kinematics_observe(const HwyHighwayParams& P, co
     const double xr = 5.0 * kMaxSpeed, yr = 4.0 * P.lanes_count, vr = 2 * kMaxSpeed;
     int row = -1;
     double r1 = 0, r2 = 0, r3 = 0, r4 = 0;
-    if (i == 0) {
+    if (i == o) {
         row = 0;
         r1 = ex;
         r2 = ey;
@@ -944,6 +945,55 @@ __device__ __forceinline__ void apply_collisions(EnvShared<TPE>& sm, const Frame
     }
 }
 
+// ------------------------------------------------------------------ several controlled vehicles
+// Per-env shared staging of the multi-agent step kernel, placed after the block's EnvShared array (so EnvShared and
+// the single-agent kernels keep their layout): the slots whose kind is MDPVehicle or Vehicle, in slot order.
+template <int TPE>
+struct MultiShared {
+    uint32_t ego[TPE / 32];
+};
+
+// Slot of the a-th set bit of an env's controlled-vehicle mask (slot 0 when there are fewer).
+template <int NW>
+__device__ __forceinline__ int nth_controlled(const uint32_t (&m)[NW], int a) {
+    for (int w = 0; w < NW; ++w) {
+        uint32_t b = m[w];
+        const int c = __popc(b);
+        if (a < c) {
+            for (; a > 0; --a) b &= b - 1;
+            return w * 32 + __ffs(b) - 1;
+        }
+        a -= c;
+    }
+    return 0;
+}
+
+// The spawn layout of HighwayEnv._create_vehicles with A controlled vehicles (envs/highway_env.py:72-98): bin k of
+// near_split(V - A, num_bins=A) (utils.py:355: the quotient, + 1 for the first `remainder` bins) is controlled vehicle k
+// followed by that bin's traffic.  Returns the bin of slot v, i.e. its agent index when `ego` (v opens the bin); the
+// controlled slots below v are bin + !ego.  v = V gives (A, true).
+__host__ __device__ __forceinline__ int spawn_bin(int V, int A, int v, bool& ego) {
+    const int q = (V - A) / A, r = (V - A) % A, big = r * (q + 2);
+    const int bin = v < big ? v / (q + 2) : r + (v - big) / (q + 1);
+    ego = (v < big ? v % (q + 2) : (v - big) % (q + 1)) == 0;
+    return bin;
+}
+__host__ __device__ __forceinline__ bool spawn_is_ego(int V, int A, int v) {
+    bool ego;
+    spawn_bin(V, A, v, ego);
+    return ego;
+}
+__host__ __device__ __forceinline__ int spawn_egos_before(int V, int A, int v) {
+    bool ego;
+    const int bin = spawn_bin(V, A, v, ego);
+    return bin + !ego;
+}
+// slot of controlled vehicle k
+__host__ __device__ __forceinline__ int spawn_ego_slot(int V, int A, int k) {
+    const int q = (V - A) / A, r = (V - A) % A;
+    return k * (q + 1) + min(k, r);
+}
+
 // ------------------------------------------------------------------ fused autoreset
 // PCG64 jump table: state_n = A^n * state_0 + G_n * inc (mod 2^128), G_n = sum_{j<n} A^j, so a
 // thread can enter the env's numpy stream at any output index with two 128-bit multiplies.
@@ -1005,12 +1055,13 @@ __device__ __forceinline__ void draw_linear_params(Pcg64& g, const HwyLinearTraf
 // (barriers); only envs with do_reset do work.  On return r/speed_index hold the new state.
 // LINEAR: LinearVehicle traffic draws its 5 parameters between the position and DELTA (8 outputs per
 // vehicle instead of 3) and stores them in T->params.
-template <int TPE, bool LINEAR = false>
+// MULTI: the spawn layout of spawn_bin, each controlled vehicle drawing what vehicle 0 draws.
+template <int TPE, bool LINEAR = false, bool MULTI = false>
 __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const HwyHighwayState& S,
                                             EnvShared<TPE>& sm, int e, int i, bool active,
                                             bool do_reset, bool simple_geometry, VehicleRegs& r,
                                             int& speed_index, const HwyLinearTraffic* T = nullptr) {
-    const int V = P.n_vehicles, L = P.lanes_count;
+    const int V = P.n_vehicles, L = P.lanes_count, A = P.n_agents;
     const size_t n = (size_t)S.n_envs;
     constexpr int kPer = LINEAR ? 3 + HWY_LINEAR_PARAMS : 3;  // 64-bit outputs per traffic vehicle
     auto jump = [](const Pcg64& g, int k) { return LINEAR ? pcg_at_far(g, k) : pcg_at(g, k); };
@@ -1030,13 +1081,26 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
     const int h0 = do_reset ? (int)g0.has32 : 0;
     const int n32 = L > 1 ? 1 : 0;                            // choice(1) draws nothing
     const int ego32 = (n32 && P.initial_lane_id < 0) ? 1 : 0;
-    auto q_before = [&](int k) { return k == 0 ? 0 : ego32 + (k - 1) * n32; };       // 32-bit requests before k
-    auto n64_before = [&](int k) { return k == 0 ? 0 : 1 + kPer * (k - 1); };         // 64-bit outputs before k
+    auto q_before = [&](int k) {  // 32-bit requests before k
+        if constexpr (MULTI) {
+            const int eb = spawn_egos_before(V, A, k);
+            return eb * ego32 + (k - eb) * n32;
+        }
+        return k == 0 ? 0 : ego32 + (k - 1) * n32;
+    };
+    auto n64_before = [&](int k) {  // 64-bit outputs before k
+        if constexpr (MULTI) {
+            const int eb = spawn_egos_before(V, A, k);
+            return eb + kPer * (k - eb);
+        }
+        return k == 0 ? 0 : 1 + kPer * (k - 1);
+    };
     auto fresh_before = [&](int q) { return h0 == 0 ? (q + 1) / 2 : q / 2; };         // outputs used by requests < q
     auto base_of = [&](int k) { return fresh_before(q_before(k)) + n64_before(k); };  // outputs before vehicle k
     if (do_reset && active && simple_geometry) {
         const int k = i;
-        const bool has32 = k == 0 ? ego32 : n32;
+        const bool is_ego = MULTI ? spawn_is_ego(V, A, k) : k == 0;
+        const bool has32 = is_ego ? ego32 : n32;
         Pcg64 g = jump(g0, base_of(k));
         uint32_t r32 = 0;
         if (has32) {
@@ -1046,8 +1110,12 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
             } else if (rq == 0) {
                 r32 = g0.u32;                // the half buffered before this reset
             } else {
-                // high half of the output the previous requester opened: vehicle k-1
-                Pcg64 gp = jump(g0, base_of(k - 1));
+                // high half of the output the previous requester opened: vehicle k-1 (MULTI: the last one before k
+                // that draws a lane; controlled vehicles with an initial_lane_id do not)
+                int kp = k - 1;
+                if constexpr (MULTI)
+                    while (kp > 0 && !(spawn_is_ego(V, A, kp) ? ego32 : n32)) --kp;
+                Pcg64 gp = jump(g0, base_of(kp));
                 r32 = (uint32_t)(gp.next64() >> 32);
             }
             // Lemire (random_bounded_uint64, rng = L-1): rejection => serial fallback
@@ -1057,9 +1125,8 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
                 sm.sp_fallback = 1;
             lane_id = (int)(m >> 32);
         }
-        if (k == 0 && P.initial_lane_id >= 0) lane_id = P.initial_lane_id;
+        if (is_ego && P.initial_lane_id >= 0) lane_id = P.initial_lane_id;
         const HwyStraightLane& Ln = P.lanes[lane_id];
-        const bool is_ego = k == 0;
         speed = is_ego ? P.ego_speed : g.uniform(0.7 * Ln.speed_limit, 0.8 * Ln.speed_limit);
         double spacing = is_ego ? P.ego_spacing : 1 / P.vehicles_density;
         double default_spacing = 12 + 1.0 * speed;
@@ -1069,7 +1136,7 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
             if (!is_ego) draw_linear_params(g, *T, lin);
         }
         if (!is_ego) delta = g.uniform(P.delta_lo, P.delta_hi);
-        sm.sp_x[k] = is_ego ? 3 * offset + incr : incr;  // x0 = 3 * offset; x0 += offset * U
+        sm.sp_x[k] = k == 0 ? 3 * offset + incr : incr;  // x0 = 3 * offset; x0 += offset * U
     }
     env_sync<TPE>();
     if (do_reset && i == 0) {
@@ -1081,7 +1148,7 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
                 sm.sp_x[k] = x;
             }
             // stream position after the reset
-            const int Q = ego32 + (V - 1) * n32;
+            const int Q = MULTI ? q_before(V) : ego32 + (V - 1) * n32;  // 32-bit requests of the whole spawn
             Pcg64 ge = jump(g0, fresh_before(Q) + n64_before(V));
             uint32_t has_f = (uint32_t)((h0 + Q) & 1), u_f = g0.u32;
             if (Q > 0) {
@@ -1089,6 +1156,15 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
                 if (((h0 + rf) & 1) != 0) rf -= 1;
                 if (rf >= 0) {
                     int kf = ego32 ? rf : rf + 1;  // vehicle issuing request rf
+                    if constexpr (MULTI) {
+                        for (int v = 0, q = 0; v < V; ++v) {
+                            if (!(spawn_is_ego(V, A, v) ? ego32 : n32)) continue;
+                            if (q++ == rf) {
+                                kf = v;
+                                break;
+                            }
+                        }
+                    }
                     Pcg64 gp = jump(g0, base_of(kf));
                     u_f = (uint32_t)(gp.next64() >> 32);
                 }
@@ -1107,7 +1183,7 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
         double2* hs = reinterpret_cast<double2*>(S.hs);
         const size_t base = (size_t)e * S.vp;
         for (int v = 0; v < V; ++v) {
-            const bool is_ego = v == 0;
+            const bool is_ego = MULTI ? spawn_is_ego(V, A, v) : v == 0;
             int id = (is_ego && P.initial_lane_id >= 0) ? P.initial_lane_id : g.choice(L);
             const HwyStraightLane& Lv = P.lanes[id];
             double sp = is_ego ? P.ego_speed : g.uniform(0.7 * Lv.speed_limit, 0.8 * Lv.speed_limit);
@@ -1139,7 +1215,7 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
     }
     env_sync<TPE>();
     if (do_reset && active) {
-        const bool is_ego = i == 0;
+        const bool is_ego = MULTI ? spawn_is_ego(V, A, i) : i == 0;
         double px, py, heading;
         if (fallback) {
             const size_t slot = (size_t)e * S.vp + i;  // staged by thread 0 before the barrier
@@ -1227,7 +1303,7 @@ highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighway
                     uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
                     double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
                     const int autoreset, float* __restrict__ final_obs, const int dense_epb) {
-    constexpr bool LINEAR = false;
+    constexpr bool LINEAR = false, MULTI = false;
     const HwyLinearTraffic* T = nullptr;
 #include "hwy_highway_step.cuh"
 }
@@ -1241,7 +1317,7 @@ highway_linear_step_kernel(const __grid_constant__ HwyHighwayParams P, const Hwy
                            uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
                            double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
                            const int autoreset, float* __restrict__ final_obs, const int dense_epb) {
-    constexpr bool LINEAR = true;
+    constexpr bool LINEAR = true, MULTI = false;
     const HwyLinearTraffic* T = &T_;
 #include "hwy_highway_step.cuh"
 }
@@ -1284,7 +1360,7 @@ highway_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHigh
 __global__ void __launch_bounds__(128)
 highway_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                      const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
-    constexpr bool LINEAR = false;
+    constexpr bool LINEAR = false, MULTI = false;
     const HwyLinearTraffic* T = nullptr;
 #include "hwy_highway_reset.cuh"
 }
@@ -1293,7 +1369,7 @@ __global__ void __launch_bounds__(128)
 highway_linear_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                             const __grid_constant__ HwyLinearTraffic T_, const uint8_t* __restrict__ mask_a,
                             const uint8_t* __restrict__ mask_b) {
-    constexpr bool LINEAR = true;
+    constexpr bool LINEAR = true, MULTI = false;
     const HwyLinearTraffic* T = &T_;
 #include "hwy_highway_reset.cuh"
 }
@@ -1381,6 +1457,72 @@ __global__ void debug_pcg64_kernel(int op, int arg_i, double arg_lo, double arg_
     store_rng_all(words_out, (size_t)n, e, g);
 }
 
+
+// ------------------------------------------------------------------ multi-agent kernels
+// (defined after every other kernel of the library, so that the single-agent kernels compile to the same code)
+// Several controlled vehicles (P.n_agents > 1, IDMVehicle traffic; see HwyHighwayParams.n_agents): every controlled
+// slot takes its own action on frame 0, the Kinematics epilogue runs once per observer under multi_obs, and the fused
+// autoreset spawns the multi-agent layout (spawn_bin).  Lane tables are always congruent (AL) on this path.  The
+// block's MultiShared staging follows its EnvShared array in dynamic shared memory.
+template <int TPE, bool DENSE>
+__global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
+highway_multi_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
+                          const int32_t* __restrict__ action_i, const float* __restrict__ action_f,
+                          float* __restrict__ obs, double* __restrict__ reward,
+                          uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated,
+                          double* __restrict__ info_speed, uint8_t* __restrict__ info_crashed,
+                          const int autoreset, float* __restrict__ final_obs, const int dense_epb) {
+    constexpr bool LINEAR = false, MULTI = true, AL = true;
+    const HwyLinearTraffic* T = nullptr;
+#include "hwy_highway_step.cuh"
+}
+
+// highway_observe_kernel with several controlled vehicles (P.n_agents > 1): under multi_obs one observation per controlled vehicle
+// as observer, obs [n_envs][n_agents][K][columns]; otherwise the first controlled vehicle's.
+template <int TPE>
+__global__ void __launch_bounds__(TPE == 32 ? 128 : TPE)
+highway_multi_observe_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
+                             const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b,
+                             float* __restrict__ obs) {
+    constexpr int EPB = TPE == 32 ? 4 : 1;
+    __shared__ ObsShared<TPE> smem[EPB];
+    const int sub = threadIdx.x / TPE, i = threadIdx.x % TPE;
+    const int env = blockIdx.x * EPB + sub;
+    const bool env_ok = env < S.n_envs;
+    const int e = env_ok ? env : S.n_envs - 1;
+    ObsShared<TPE>& sm = smem[sub];
+    const int V = P.n_vehicles;
+    const bool active = i < V;
+    VehicleRegs r;
+    load_vehicle(S, (size_t)e * S.vp + (active ? i : 0), r);
+    publish(P, sm.f, i, active, r);
+    env_sync<TPE>();
+    const bool wanted = env_ok && env_selected(mask_a, mask_b, e);
+    const int NA = P.multi_obs ? P.n_agents : 1;
+    const size_t per = (size_t)P.obs_vehicles_count * obs_columns(P);
+    for (int a = 0, seen = 0, o = 0; a < NA; ++a) {
+        // slot of controlled vehicle a (list order)
+        for (; o < V; ++o) {
+            const int k = meta_kind(S.meta[(size_t)e * S.vp + o]);
+            if ((k == HWY_KIND_MDP || k == HWY_KIND_VEHICLE) && seen++ == a) break;
+        }
+        const int obs_slot = o < V ? o : 0;
+        kinematics_observe(P, sm.f, sm.key, i, r.heading, wanted ? obs + ((size_t)e * NA + a) * per : nullptr,
+                           nullptr, obs_slot);
+        if (o < V) ++o;
+        env_sync<TPE>();  // the next observer's keys overwrite sm.key
+    }
+}
+
+// several controlled vehicles (P.n_agents > 1): the spawn layout of spawn_bin
+__global__ void __launch_bounds__(128)
+highway_multi_reset_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
+                           const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
+    constexpr bool LINEAR = false, MULTI = true;
+    const HwyLinearTraffic* T = nullptr;
+#include "hwy_highway_reset.cuh"
+}
+
 }  // namespace hwy
 
 // ====================================================================== C ABI
@@ -1422,6 +1564,8 @@ int validate(const HwyHighwayParams* p, const HwyHighwayState* s) {
             return fail("%s", "unknown observation feature code");
     if (p->n_target_speeds < 1 || p->n_target_speeds > HWY_MAX_TARGET_SPEEDS)
         return fail("%s", "n_target_speeds out of range");
+    if (p->n_agents < 0 || p->n_agents > 8) return fail("%s", "n_agents out of range (0..8)");
+    if (p->n_agents > p->n_vehicles) return fail("%s", "n_agents exceeds n_vehicles");
     if (p->simulation_frequency < 1 || p->policy_frequency < 1 ||
         p->simulation_frequency < p->policy_frequency)
         return fail("%s", "bad simulation/policy frequency");
@@ -1590,6 +1734,15 @@ int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const ui
                    const uint8_t* mask_b, float* obs, cudaStream_t st) {
     int tpe = tpe_for(p->n_vehicles);
     Grid g = grid_for(tpe, s->n_envs);
+    if (p->n_agents > 1) {
+        if (tpe == 32)
+            hwy::highway_multi_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
+        else if (tpe == 64)
+            hwy::highway_multi_observe_kernel<64><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
+        else
+            hwy::highway_multi_observe_kernel<128><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
+        return check_launch("highway_multi_observe_kernel");
+    }
     if (tpe == 32)
         hwy::highway_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
     else if (tpe == 64)
@@ -1603,6 +1756,10 @@ int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const ui
 int launch_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
                  const uint8_t* mask_a, const uint8_t* mask_b, cudaStream_t st) {
     int blocks = (s->n_envs + 127) / 128;
+    if (p->n_agents > 1) {
+        hwy::highway_multi_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, mask_a, mask_b);
+        return check_launch("highway_multi_reset_kernel");
+    }
     if (t) {
         hwy::highway_linear_reset_kernel<<<blocks, 128, 0, st>>>(*p, *s, *t, mask_a, mask_b);
         return check_launch("highway_linear_reset_kernel");
@@ -1623,6 +1780,10 @@ int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const i
     return 0;
 }
 
+int dispatch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                        const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                        double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st);
+
 int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
                   const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
                   uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
@@ -1631,6 +1792,12 @@ int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const Hwy
     // HWYB200_GENERAL_LANES=1 (tests): run the general-geometry instantiation on a congruent lane table too
     const char* force_general = getenv("HWYB200_GENERAL_LANES");
     const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
+    if (p->n_agents > 1) {
+        if (!al) return fail("%s", "several controlled vehicles need a congruent lane table (no general-geometry "
+                                   "multi-agent kernel)");
+        return dispatch_multi_step(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
+                                   info_crashed, autoreset, final_obs, st);
+    }
 #define HWY_LAUNCH_STEP(T, A)                                                                              \
     launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
                       autoreset, final_obs, st)
@@ -1645,6 +1812,54 @@ int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const Hwy
     if (rc) return 1;
     if (check_launch(t ? "highway_linear_step_kernel" : "highway_step_kernel")) return 1;
     return 0;
+}
+// Several controlled vehicles (n_agents > 1): highway_multi_step_kernel, on congruent lane tables only.
+template <int TPE>
+int launch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                      const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                      double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st) {
+    if (autoreset > 0 && ensure_pcg_jump(st)) return 1;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
+    const size_t env_bytes = sizeof(hwy::EnvShared<TPE>) + sizeof(hwy::MultiShared<TPE>);
+    const int epb = step_envs_per_block(p->n_vehicles, env_bytes, s->n_envs, step_device(dev));
+    const bool dense = epb * TPE > step_half_block_threads();
+    const int blocks = (s->n_envs + epb - 1) / epb;
+    const size_t smem = (size_t)epb * env_bytes;
+    static std::atomic<size_t> configured[2][64];
+    if (smem > configured[dense][dev].load(std::memory_order_relaxed)) {
+        cudaError_t err = dense ? cudaFuncSetAttribute(hwy::highway_multi_step_kernel<TPE, true>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                                : cudaFuncSetAttribute(hwy::highway_multi_step_kernel<TPE, false>,
+                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
+        configured[dense][dev].store(smem, std::memory_order_relaxed);
+    }
+    if (dense)
+        hwy::highway_multi_step_kernel<TPE, true><<<blocks, (epb * p->n_vehicles + 31) & ~31, smem, st>>>(
+            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, autoreset,
+            final_obs, epb);
+    else
+        hwy::highway_multi_step_kernel<TPE, false><<<blocks, epb * TPE, smem, st>>>(
+            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, autoreset,
+            final_obs, epb);
+    return check_launch("highway_multi_step_kernel");
+}
+
+// (after dispatch_step: the multi-agent kernels are instantiated after every single-agent one, whose code and
+// constant-bank layout then stay as they were)
+int dispatch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
+                        const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                        double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st) {
+    const int tpe = tpe_for(p->n_vehicles);
+    if (tpe == 32)
+        return launch_multi_step<32>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
+                                     info_crashed, autoreset, final_obs, st);
+    if (tpe == 64)
+        return launch_multi_step<64>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
+                                     info_crashed, autoreset, final_obs, st);
+    return launch_multi_step<128>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
+                                  info_crashed, autoreset, final_obs, st);
 }
 }  // namespace
 
@@ -1665,6 +1880,7 @@ int hwy_highway_reset(const HwyHighwayParams* p, const HwyHighwayState* s, const
                       const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
     if (t && !t->params) return fail("%s", "null linear traffic parameters");
     if (validate(p, s)) return 1;
+    if (t && p->n_agents > 1) return fail("%s", "LinearVehicle traffic with several controlled vehicles");
     cudaStream_t st = (cudaStream_t)stream;
     if (ensure_pcg_jump(st)) return 1;  // the fused autoreset of later steps reads the table
     if (launch_reset(p, s, t, mask_a, mask_b, st)) return 1;
@@ -1718,6 +1934,7 @@ int hwy_highway_step(const HwyHighwayParams* p, const HwyHighwayState* s, const 
                      int autoreset, float* final_obs, void* stream) {
     if (t && !t->params) return fail("%s", "null linear traffic parameters");
     if (check_step_args(p, s, action_i, action_f, obs, reward, terminated, truncated, autoreset)) return 1;
+    if (t && p->n_agents > 1) return fail("%s", "LinearVehicle traffic with several controlled vehicles");
     return dispatch_step(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
                          autoreset, final_obs, (cudaStream_t)stream);
 }
@@ -1727,6 +1944,7 @@ int hwy_highway_substeps(const HwyHighwayParams* p, const HwyHighwayState* s, co
                          int n_substeps, const float* action_f, void* stream) {
     if (t && !t->params) return fail("%s", "null linear traffic parameters");
     if (validate(p, s)) return 1;
+    if (t && p->n_agents > 1) return fail("%s", "LinearVehicle traffic with several controlled vehicles");
     if (n_substeps < 1 || n_substeps > 4096) return fail("%s", "n_substeps must be in 1..4096");
     return dispatch_step(p, s, t, nullptr, action_f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                          -n_substeps, nullptr, (cudaStream_t)stream);

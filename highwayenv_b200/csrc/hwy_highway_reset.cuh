@@ -1,5 +1,6 @@
-// hwy_highway_reset.cuh — the body of the highway reset kernels, included by highway_reset_kernel (LINEAR = false)
-// and highway_linear_reset_kernel (LINEAR = true) in hwy_highway.cu.  In scope: LINEAR, the kernel parameters and
+// hwy_highway_reset.cuh — the body of the highway reset kernels, included by highway_reset_kernel (LINEAR = false),
+// highway_linear_reset_kernel (LINEAR = true) and highway_multi_reset_kernel (MULTI = true: several controlled
+// vehicles in the layout of spawn_bin) in hwy_highway.cu.  In scope: LINEAR, MULTI, the kernel parameters and
 // `const HwyLinearTraffic* T`.
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;
@@ -18,7 +19,7 @@
     const size_t base = (size_t)e * S.vp;
     int ego_speed_index = -1;
     for (int v = 0; v < P.n_vehicles; ++v) {
-        const bool is_ego = v == 0;
+        const bool is_ego = MULTI ? spawn_is_ego(P.n_vehicles, P.n_agents, v) : v == 0;
         // choice(list(graph.keys())) / choice(list(graph[_from].keys())): single element => no draw
         int id = (is_ego && P.initial_lane_id >= 0) ? P.initial_lane_id : g.choice(P.lanes_count);
         const HwyStraightLane& L = P.lanes[id];
@@ -55,8 +56,17 @@
                 kind = HWY_KIND_MDP;
                 ego_speed_index = speed_to_index(P, target_speed);
                 target_speed = P.target_speeds[ego_speed_index];
+                if constexpr (MULTI) {
+                    bool ego;
+                    const int agent = spawn_bin(P.n_vehicles, P.n_agents, v, ego);
+                    S.speed_index[(size_t)e * P.n_agents + agent] = ego_speed_index;
+                }
             } else {
                 kind = HWY_KIND_VEHICLE;
+                if constexpr (MULTI) {
+                    bool ego;
+                    S.speed_index[(size_t)e * P.n_agents + spawn_bin(P.n_vehicles, P.n_agents, v, ego)] = -1;
+                }
             }
         } else {
             kind = HWY_KIND_IDM;
@@ -77,6 +87,6 @@
                            (cc ? HWY_META_CHECK_COLLISIONS : 0) | (kind << HWY_META_KIND_SHIFT) |
                            HWY_META_PRESENT | ((aligned ? v : 0) << HWY_META_ORDER_SHIFT);
     }
-    S.speed_index[e] = ego_speed_index;
+    if constexpr (!MULTI) S.speed_index[e] = ego_speed_index;
     S.time[e] = 0.0;
     store_rng_all(S.rng, (size_t)S.n_envs, e, g);

@@ -1,6 +1,7 @@
-// hwy_highway_step.cuh — the body of the highway step kernels, included by highway_step_kernel (LINEAR = false) and
-// highway_linear_step_kernel (LINEAR = true) in hwy_highway.cu.  In scope: TPE, AL, LINEAR, the kernel parameters
-// and `const HwyLinearTraffic* T`.  See the comment above highway_step_kernel.
+// hwy_highway_step.cuh — the body of the highway step kernels, included by highway_step_kernel (LINEAR = false),
+// highway_linear_step_kernel (LINEAR = true) and highway_multi_step_kernel (MULTI = true: several controlled
+// vehicles) in hwy_highway.cu.  In scope: TPE, AL, LINEAR, MULTI, the kernel parameters and
+// `const HwyLinearTraffic* T`.  See the comment above highway_step_kernel.
     constexpr int NW = TPE / 32;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     EnvShared<TPE>* smem = reinterpret_cast<EnvShared<TPE>*>(smem_raw);
@@ -19,6 +20,8 @@
     EnvShared<TPE>& sm = smem[sub];
     LinearShared<TPE>* lsm = nullptr;
     if constexpr (LINEAR) lsm = reinterpret_cast<LinearShared<TPE>*>(smem + EPB) + sub;
+    MultiShared<TPE>* msm = nullptr;
+    if constexpr (MULTI) msm = reinterpret_cast<MultiShared<TPE>*>(smem + EPB) + sub;
     const size_t slot = (size_t)e * S.vp + (active ? i : 0);
     const bool aligned = AL || lanes_aligned(P);
     const bool congruent = AL || lanes_congruent(P);
@@ -31,7 +34,10 @@
         load_vehicle(S, slot, r);
     }
     const int kind = meta_kind(r.meta);
-    int speed_index = (i == 0) ? S.speed_index[e] : 0;
+    int speed_index = (!MULTI && i == 0) ? S.speed_index[e] : 0;  // MULTI: read on frame 0, per controlled vehicle
+    // MULTI: this slot is a controlled vehicle (MDPVehicle or Vehicle), the agent-th one of its env
+    const bool controlled = MULTI && active && (kind == HWY_KIND_MDP || kind == HWY_KIND_VEHICLE);
+    int agent = 0;
     double act_steer = 0.0, act_accel = 0.0;
     // autoreset < 0 (hwy_highway_substeps): -autoreset times Road.act() + Road.step(dt) and nothing else — no
     // action_type.act, no observation / reward / clock; the controlled vehicle acts like ControlledVehicle.act(None)
@@ -43,8 +49,12 @@
     {
         uint32_t b_cc = __ballot_sync(0xffffffffu, active && (r.meta & HWY_META_CHECK_COLLISIONS));
         uint32_t b_ctrl = __ballot_sync(0xffffffffu, active && kind != HWY_KIND_VEHICLE);
+        uint32_t b_ego = 0;
+        if constexpr (MULTI) b_ego = __ballot_sync(0xffffffffu, controlled);
         if constexpr (DENSE) {
             if (i < NW) sm.cc[i] = sm.ctrl[i] = sm.mid[i] = 0;
+            if constexpr (MULTI)
+                if (i < NW) msm->ego[i] = 0;
             if (active) {
                 sm.last_will[i] = -1;
                 sm.crash_hit[i] = 0;
@@ -54,6 +64,7 @@
                 sm.cc[i >> 5] = b_cc;
                 sm.ctrl[i >> 5] = b_ctrl;
                 sm.mid[i >> 5] = 0;
+                if constexpr (MULTI) msm->ego[i >> 5] = b_ego;
             }
             sm.last_will[i] = -1;
             sm.crash_hit[i] = 0;
@@ -72,6 +83,7 @@
             __syncthreads();  // (once per launch) the zeroed words before the env segments OR their bits in
             segment_or(sm.cc, b_cc, i, V);
             segment_or(sm.ctrl, b_ctrl, i, V);
+            if constexpr (MULTI) segment_or(msm->ego, b_ego, i, V);
         }
     }
     const IdmK K = make_idm(P);
@@ -115,28 +127,48 @@
 
         // ---- action_type.act(action) on the first frame (abstract.py:294-304)
         if (frame == 0) {
-            if (i == 0) {
+            if constexpr (MULTI) {  // (the ego mask is complete: two barriers since the static masks)
+                for (int w = 0; w < NW; ++w)
+                    agent += __popc(w < (i >> 5) ? msm->ego[w] : (w == (i >> 5) ? msm->ego[w] & ((1u << (i & 31)) - 1u) : 0u));
+                if (controlled && agent < P.n_agents) speed_index = S.speed_index[(size_t)e * P.n_agents + agent];
+            }
+            // MULTI: MultiAgentAction hands action k to controlled vehicle k (action.py:301-333); a plain action type
+            // acts on the first one only, the others act(None) (abstract.py:294-304, Road.act)
+            // (a controlled slot past the n_agents-th, which only a hand-made state has, acts(None) and keeps no index)
+            const bool own_action = MULTI && agent < P.n_agents && (P.multi_action || agent == 0);
+            const size_t act_row = MULTI && P.multi_action ? (size_t)e * P.n_agents + agent : (size_t)e;
+            if (MULTI ? controlled : i == 0) {
                 if (kind == HWY_KIND_MDP) {
                     // MDPVehicle.act (controller.py:295-315) + ControlledVehicle.act lane part
                     // (:99-124); labels action.py:204.  follow_road (:135-143) cannot change the
                     // target on the single-road highway graph (next_lane hits KeyError,
                     // road/road.py:129-130).
-                    int a = substeps_only ? 1 : action_i[e];  // substeps only: act(None) = IDLE
+                    int a;
+                    if constexpr (MULTI)
+                        a = (substeps_only || !own_action) ? 1 : action_i[act_row];
+                    else
+                        a = substeps_only ? 1 : action_i[e];  // substeps only: act(None) = IDLE
                     if (a == 3 || a == 4) {
                         int idx = speed_to_index(P, r.speed) + (a == 3 ? 1 : -1);
                         idx = max(0, min(idx, P.n_target_speeds - 1));
                         speed_index = idx;
                         r.target_speed = P.target_speeds[idx];
-                        F.ts[0] = r.target_speed;
+                        F.ts[MULTI ? i : 0] = r.target_speed;
                     } else if (a == 0 || a == 2) {
                         int old = meta_target(r.meta);
                         int id = old + (a == 2 ? 1 : -1);
                         id = max(0, min(id, P.lanes_count - 1));
                         if (lane_reachable(P.lanes[id], r.x, r.y)) {
                             r.meta = meta_set_target(r.meta, id);
-                            F.tgt[0] = (unsigned char)id;
-                            F.tm[old][0] &= ~1u;
-                            F.tm[id][0] |= 1u;
+                            if constexpr (MULTI) {  // (several controlled vehicles may share a mask word)
+                                F.tgt[i] = (unsigned char)id;
+                                atomicAnd(&F.tm[old][i >> 5], ~(1u << (i & 31)));
+                                atomicOr(&F.tm[id][i >> 5], 1u << (i & 31));
+                            } else {
+                                F.tgt[0] = (unsigned char)id;
+                                F.tm[old][0] &= ~1u;
+                                F.tm[id][0] |= 1u;
+                            }
                         }
                     }
                 } else {
@@ -144,7 +176,8 @@
                     // lmap (utils.py:31-33) stays in float32 (NEP 50 weak python scalars)
                     // (substeps only: the vehicle's current action dict, or the default {0, 0} when none is given —
                     // lmap(0) of the symmetric default ranges)
-                    float a0 = action_f ? action_f[2 * (size_t)e] : 0.0f, a1 = action_f ? action_f[2 * (size_t)e + 1] : 0.0f;
+                    const size_t row = MULTI ? act_row : (size_t)e;
+                    float a0 = action_f ? action_f[2 * row] : 0.0f, a1 = action_f ? action_f[2 * row + 1] : 0.0f;
                     if (P.act_clip) {
                         a0 = fminf(fmaxf(a0, -1.0f), 1.0f);
                         a1 = fminf(fmaxf(a1, -1.0f), 1.0f);
@@ -157,6 +190,10 @@
                                                              (float)(P.steer_hi - P.steer_lo)), 2.0f));
                     act_accel = (double)acc;
                     act_steer = (double)st;
+                    if (MULTI && !own_action) {  // Vehicle.act(None) keeps the action dict it was created with
+                        act_accel = 0.0;
+                        act_steer = 0.0;
+                    }
                 }
             }
             env_sync<TPE>();
@@ -425,6 +462,18 @@
     const Frame<TPE>& F = sm.f[p];
     const size_t obs_off = (size_t)e * P.obs_vehicles_count * obs_columns(P);
     float* obs_env = obs + obs_off;
+    // MULTI: one observation per controlled vehicle as observer under multi_obs (observation.py:588-604), else the
+    // first one's; rows [n_envs][NA][K][columns]
+    const int NA = MULTI && P.multi_obs ? P.n_agents : 1;
+    if constexpr (MULTI) {
+        for (int a = 0; a < NA; ++a) {
+            const size_t off = ((size_t)e * NA + a) * P.obs_vehicles_count * obs_columns(P);
+            kinematics_observe<TPE, DENSE>(P, F, sm.key, i, r.heading, env_ok ? obs + off : nullptr,
+                                           (autoreset && final_obs) ? final_obs + off : nullptr,
+                                           nth_controlled(msm->ego, a));
+            env_sync<TPE>();  // the next observer's keys overwrite sm.key
+        }
+    } else
     kinematics_observe<TPE, DENSE>(P, F, sm.key, i, r.heading, env_ok ? obs_env : nullptr,
                        (autoreset && final_obs) ? final_obs + obs_off : nullptr);
     if (i == 0) {
@@ -453,7 +502,7 @@
         rew *= on_road ? 1.0 : 0.0;
         double t = S.time[e] + 1.0 / P.policy_frequency;  // abstract.py:274
         S.time[e] = t;
-        S.speed_index[e] = speed_index;
+        if constexpr (!MULTI) S.speed_index[e] = speed_index;
         reward[e] = rew;
         terminated[e] = (uint8_t)(is_crashed || (P.offroad_terminal && !on_road));
         truncated[e] = (uint8_t)(t >= P.duration);
@@ -469,13 +518,15 @@
         }
         sm.done = autoreset && (is_crashed || (P.offroad_terminal && !on_road) || t >= P.duration);
     }
+    if constexpr (MULTI)
+        if (controlled && env_ok && agent < P.n_agents) S.speed_index[(size_t)e * P.n_agents + agent] = speed_index;
     if (autoreset) {
         // ---- SameStep autoreset fused into the step: envs that ended re-spawn from their own
         // numpy stream and return the reset observation (gymnasium AutoresetMode.SAME_STEP)
         env_sync<TPE>();
         const bool do_reset = env_ok && sm.done;
         const bool simple_geometry = aligned && P.lanes[0].start_x == 0.0 && P.lanes[0].dir_x == 1.0;
-        spawn_fused<TPE, LINEAR>(P, S, sm, e, i, active, do_reset, simple_geometry, r, speed_index, T);
+        spawn_fused<TPE, LINEAR, MULTI>(P, S, sm, e, i, active, do_reset, simple_geometry, r, speed_index, T);
         Frame<TPE>& G = sm.f[p ^ 1];
         if (do_reset) publish<TPE, false, DENSE>(P, G, i, active, r);
         // barrier + "does any env of this block re-spawn?": the second observation runs under a block-uniform
@@ -483,10 +534,23 @@
         // __syncthreads() is what compute-sanitizer's synccheck rejects, even though the arrival counts match)
         const bool any_reset = __syncthreads_or(do_reset) != 0;
         if (any_reset) {
+            if constexpr (MULTI) {  // the respawned layout: controlled vehicle a at spawn_ego_slot(a)
+                for (int a = 0; a < NA; ++a) {
+                    const size_t off = ((size_t)e * NA + a) * P.obs_vehicles_count * obs_columns(P);
+                    kinematics_observe<TPE, DENSE>(P, G, sm.key, i, r.heading, do_reset ? obs + off : nullptr,
+                                                   nullptr, spawn_ego_slot(V, P.n_agents, a));
+                    env_sync<TPE>();
+                }
+                if (do_reset && i == 0) S.time[e] = 0.0;
+                bool ego;
+                const int ag = spawn_bin(V, P.n_agents, i, ego);
+                if (do_reset && active && ego) S.speed_index[(size_t)e * P.n_agents + ag] = speed_index;
+            } else {
             kinematics_observe<TPE, DENSE>(P, G, sm.key, i, r.heading, do_reset ? obs_env : nullptr);
             if (do_reset && i == 0) {
                 S.time[e] = 0.0;
                 S.speed_index[e] = speed_index;
+            }
             }
         }
     }

@@ -40,8 +40,9 @@ class HostStepper:
         if self._n_table:
             if getattr(env, "_action_table", None) is None or env._action_table.device != dev:
                 env._action_table = torch.from_numpy(table).to(dev)  # env.step builds it lazily; not under capture
-            self._h_actions = torch.empty((env.num_envs,), dtype=torch.int64).pin_memory()
-            self._d_actions = torch.empty((env.num_envs,), dtype=torch.int64, device=dev)
+            shape = tuple(env._action_buf.shape[:-1])  # one index per env (and per agent under MultiAgentAction)
+            self._h_actions = torch.empty(shape, dtype=torch.int64).pin_memory()
+            self._d_actions = torch.empty(shape, dtype=torch.int64, device=dev)
         else:
             self._h_actions = pin(env._action_buf)
             self._d_actions = env._action_buf

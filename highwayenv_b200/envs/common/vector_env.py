@@ -159,12 +159,12 @@ class BatchedVectorEnv:
                 self._action_table = torch.from_numpy(table).to(buf.device)
             idx = actions if isinstance(actions, torch.Tensor) else torch.from_numpy(np.asarray(actions))
             idx = idx.to(device=buf.device, dtype=torch.long).reshape(-1)
-            if idx.numel() != buf.shape[0]:
-                raise ValueError("one action per env")
+            if idx.numel() != buf.numel() // 2:  # (buf: [N, 2], or [N, A, 2] with one action per agent)
+                raise ValueError("one action per env" + (" and agent" if buf.dim() > 2 else ""))
             # (the check reads the device: not under CUDA-graph capture — HostStepper checks its host array instead)
             if not torch.cuda.is_current_stream_capturing() and bool(((idx < 0) | (idx >= table.shape[0])).any()):
                 raise IndexError("list index out of range")  # all_actions[action] in the reference
-            torch.index_select(self._action_table, 0, idx, out=buf)
+            torch.index_select(self._action_table, 0, idx, out=buf.view(-1, 2))
             return buf
         if isinstance(actions, torch.Tensor):
             if actions.device == buf.device and actions.dtype == buf.dtype and actions.is_contiguous() \

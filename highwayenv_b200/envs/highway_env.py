@@ -22,7 +22,7 @@ import numpy as np
 import torch
 
 from .. import _native as N
-from ..spaces import batch_space
+from ..spaces import Box, batch_space
 from .common.action import action_factory
 from .common.observation import KinematicObservation, observation_factory
 from .common.vector_env import BatchedVectorEnv
@@ -59,12 +59,32 @@ class BatchedHighwayEnv(BatchedVectorEnv):
     PERCEPTION_DISTANCE = 5.0 * 40.0  # abstract.py:56
     REWARD_NAMES = ("collision_reward", "right_lane_reward", "high_speed_reward", "on_road_reward")  # _rewards :118-137
     _allocated_for = None
+    n_agents = 1
+    multi_agent = False
 
     # ------------------------------------------------------------------ configuration
     def define_spaces(self) -> None:
-        """Plugin selection by ``config[...]["type"]`` (abstract.py:154-161)."""
-        self.observation_type = observation_factory(self, self.config["observation"])
-        self.action_type = action_factory(self, self.config["action"])
+        """Plugin selection by ``config[...]["type"]`` (abstract.py:154-161).
+
+        ``config["controlled_vehicles"]`` = A > 1 spawns A controlled vehicles (highway_env.py:72-98).
+        MultiAgentAction / MultiAgentObservation (action.py:301-333, observation.py:588-604) wrap one plugin per
+        controlled vehicle; their tuples become a leading agent axis here: actions [N, A] (DiscreteMetaAction,
+        DiscreteAction) or [N, A, 2] (ContinuousAction), observations [N, A, ...].  The two switches are independent:
+        a plain action type drives the first controlled vehicle only, a plain observation observes from it only."""
+        cfg = self.config
+        act_cfg, obs_cfg = cfg["action"], cfg["observation"]
+        self.n_agents = int(cfg.get("controlled_vehicles", 1))
+        if not 1 <= self.n_agents <= 8:
+            raise ValueError("controlled_vehicles must be in 1..8")
+        self.multi_action = act_cfg["type"] == "MultiAgentAction"
+        self.multi_obs = obs_cfg["type"] == "MultiAgentObservation"
+        if self.multi_action:
+            act_cfg = act_cfg["action_config"]
+        if self.multi_obs:
+            obs_cfg = obs_cfg["observation_config"]
+        self.multi_agent = self.multi_action or self.multi_obs
+        self.observation_type = observation_factory(self, obs_cfg)
+        self.action_type = action_factory(self, act_cfg)
         # the step kernel's own epilogue is Kinematics; any other plugin runs its standalone kernel after the step
         # (envs/common/observation.py) while the kernel writes default Kinematics rows into a scratch buffer
         self._plugin_standalone = self.observation_type.standalone
@@ -76,19 +96,34 @@ class BatchedHighwayEnv(BatchedVectorEnv):
             self.observation_type.bind(self.config["policy_frequency"], self.action_type.target_speeds)
         self.single_observation_space = self.observation_type.space()
         self.single_action_space = self.action_type.space()
+        A = self.n_agents
+        if self.multi_obs:
+            per = self.single_observation_space
+            self.agent_observation_space = per
+            self.single_observation_space = Box(low=per.low.min() if per.low.size else -np.inf,
+                                                high=per.high.max() if per.high.size else np.inf,
+                                                shape=(A,) + tuple(per.shape), dtype=per.dtype)
+        if self.multi_action:
+            per = self.single_action_space
+            self.agent_action_space = per
+            if hasattr(per, "n"):  # DiscreteMetaAction / DiscreteAction index per agent
+                self.single_action_space = Box(low=0, high=per.n - 1, shape=(A,), dtype=np.int64)
+            else:
+                self.single_action_space = Box(-1.0, 1.0, shape=(A, 2), dtype=np.float32)
         self.observation_space = batch_space(self.single_observation_space, self.num_envs)
         self.action_space = batch_space(self.single_action_space, self.num_envs)
         self._params = self._build_params()
 
     def _build_params(self) -> N.HwyHighwayParams:
         cfg = self.config
-        if cfg.get("controlled_vehicles", 1) != 1:
-            raise NotImplementedError("controlled_vehicles != 1 (multi-agent) is not on the accelerated path")
+        A = self.n_agents
         ovt = cfg.get("other_vehicles_type")
         if ovt != IDM_VEHICLE and ovt not in LINEAR_VEHICLE_TYPES:
             raise NotImplementedError("only IDMVehicle and LinearVehicle / AggressiveVehicle / DefensiveVehicle traffic "
                                       "is on the accelerated path")
         self._linear = ovt in LINEAR_VEHICLE_TYPES
+        if self._linear and A > 1:
+            raise NotImplementedError("LinearVehicle traffic with several controlled vehicles")
         if cfg.get("neighbour_vehicles_connected_lanes"):
             raise NotImplementedError("connected-lane neighbour search (v1/v2 ids) is not implemented")
         if cfg.get("manual_control"):
@@ -98,9 +133,13 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         if not 1 <= lanes <= N.HWY_MAX_LANES:
             raise ValueError(f"lanes_count must be in 1..{N.HWY_MAX_LANES}")
         p.lanes_count = lanes
-        p.n_vehicles = int(cfg["vehicles_count"]) + 1
+        p.n_vehicles = int(cfg["vehicles_count"]) + A
         if p.n_vehicles > N.HWY_MAX_VEHICLES:
-            raise ValueError(f"vehicles_count must be <= {N.HWY_MAX_VEHICLES - 1}")
+            raise ValueError(f"vehicles_count + controlled_vehicles must be <= {N.HWY_MAX_VEHICLES}")
+        # one controlled vehicle (A = 1) runs the single-agent kernels whatever the switches: same layout and draws
+        p.n_agents = A if A > 1 else 0
+        p.multi_action = int(self.multi_action and A > 1)
+        p.multi_obs = int(self.multi_obs and A > 1 and not self._plugin_standalone)
         p.simulation_frequency = int(cfg["simulation_frequency"])
         p.policy_frequency = int(cfg["policy_frequency"])
         p.others_check_collisions = int(self.OTHERS_CHECK_COLLISIONS)
@@ -153,8 +192,10 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         vp = int(self._lib.hwy_highway_slot_stride(V))
         K = int(self._params.obs_vehicles_count)
         F = int(self._params.obs_n_features) or 5
-        plugin_shape = tuple(self.single_observation_space.shape) if self._plugin_standalone else None
-        key = (n, vp, K, F, int(self._params.action_type), plugin_shape, self._linear)
+        plugin_shape = tuple(self.observation_type.space().shape) if self._plugin_standalone else None  # per agent
+        A = self.n_agents
+        key = (n, vp, K, F, int(self._params.action_type), plugin_shape, self._linear, A, self.multi_action,
+               self.multi_obs)
         if self._allocated_for == key:
             return
         z = lambda *shape, dtype: torch.zeros(*shape, dtype=dtype, device=dev)  # noqa: E731
@@ -165,15 +206,19 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         self._imp = z(n, vp, 2, dtype=torch.float64)
         self._delta = z(n, vp, dtype=torch.float64)
         self._meta = z(n, vp, dtype=torch.int32)
-        self._speed_index = z(n, dtype=torch.int32)
+        self._speed_index = z(n, A, dtype=torch.int32) if A > 1 or self.multi_agent else z(n, dtype=torch.int32)
         self._time = z(n, dtype=torch.float64)
-        self._fused_out = z(n, K, F, dtype=torch.float32)  # what the step / reset kernels write
+        # what the step / reset kernels write (under MultiAgentObservation one Kinematics block per agent)
+        KA = (A,) if self.multi_obs else ()
+        self._fused_out = z(n, *KA, K, F, dtype=torch.float32) if plugin_shape is None else z(n, K, F, dtype=torch.float32)
         if plugin_shape is None:
             self._obs = self._fused_out
-            self._final_obs = z(n, K, F, dtype=torch.float32)
+            self._final_obs = z(n, *KA, K, F, dtype=torch.float32)
         else:
-            self._obs = z(n, *plugin_shape, dtype=torch.float32)
-            self._final_obs = z(n, *plugin_shape, dtype=torch.float32)
+            self._obs = z(n, *KA, *plugin_shape, dtype=torch.float32)
+            self._final_obs = z(n, *KA, *plugin_shape, dtype=torch.float32)
+        # TimeToCollision observing the first of several controlled vehicles reads its speed index from here
+        self._speed_index0 = z(n, dtype=torch.int32) if A > 1 and not self.multi_obs else None
         self._plugin_view = None
         self._reward = z(n, dtype=torch.float64)
         self._terminated = z(n, dtype=torch.uint8)
@@ -181,10 +226,11 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         self._info_speed = z(n, dtype=torch.float64)
         self._info_crashed = z(n, dtype=torch.uint8)
         self._reward_terms = z(n, N.HWY_REWARD_TERMS, dtype=torch.float64)
+        AA = (A,) if self.multi_action else ()
         if self._params.action_type == 0:
-            self._action_buf = z(n, dtype=torch.int32)
+            self._action_buf = z(n, *AA, dtype=torch.int32)
         else:
-            self._action_buf = z(n, 2, dtype=torch.float32)
+            self._action_buf = z(n, *AA, 2, dtype=torch.float32)
         st = N.HwyHighwayState()
         st.n_envs, st.vp = n, vp
         st.pos, st.hs, st.tt, st.imp = (t.data_ptr() for t in (self._pos, self._hs, self._tt, self._imp))
@@ -255,11 +301,23 @@ class BatchedHighwayEnv(BatchedVectorEnv):
             self._plugin_graph = torch.from_numpy(
                 np.frombuffer(bytes(net.to_struct()), dtype=np.uint8).copy()).to(self.device)
             v = N.HwyObsView()
-            v.n_envs, v.vp, v.n_vehicles, v.n_agents = self.num_envs, self.vp, self.V, 0
+            multi_obs = self.multi_obs and self.n_agents > 1
+            v.n_envs, v.vp, v.n_vehicles, v.n_agents = self.num_envs, self.vp, self.V, self.n_agents if multi_obs else 0
             v.pos, v.hs, v.meta = self._pos.data_ptr(), self._hs.data_ptr(), self._meta.data_ptr()
-            v.speed_index = self._speed_index.data_ptr()
+            si = self._speed_index if self._speed_index0 is None else self._speed_index0
+            v.speed_index = si.data_ptr()
             self._plugin_view = v
         return self._plugin_view, self._plugin_graph.data_ptr()
+
+    def _observe_plugin(self, out, mask_a=None, mask_b=None) -> None:
+        if self._speed_index0 is not None:  # the first controlled vehicle's column of [N, A]
+            self._speed_index0.copy_(self._speed_index[:, 0])
+        super()._observe_plugin(out, mask_a, mask_b)
+
+    def ego_slots(self) -> list:
+        """The slot of each controlled vehicle in the spawn layout of _create_vehicles (highway_env.py:72-98): bin k
+        of near_split(vehicles_count, controlled_vehicles) is controlled vehicle k followed by its traffic."""
+        return ego_slots(int(self._params.n_vehicles) - self.n_agents, self.n_agents)
 
     def get_available_actions(self) -> torch.Tensor:
         """DiscreteMetaAction.get_available_actions (envs/common/action.py:262-299, AbstractEnv.get_available_actions
@@ -271,15 +329,20 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         lanes = [self._params.lanes[k] for k in range(int(self._params.lanes_count))]
         table = torch.tensor([[L.start_x, L.start_y, L.dir_x, L.dir_y, L.lat_x, L.lat_y, L.length, L.width] for L in lanes],
                              dtype=torch.float64, device=self._pos.device)
-        lane = ((self._meta[:, 0] >> N.META_LANE_SHIFT) & 0xFF).long()
-        return available_actions_mask(self._pos[:, 0, 0], self._pos[:, 0, 1], lane, self._speed_index.long(), table,
-                                      int(self._params.n_target_speeds))
+        si = self._speed_index.view(self.num_envs, -1).long()
+        masks = []
+        for a, slot in enumerate(self.ego_slots() if self.multi_action else [0]):
+            lane = ((self._meta[:, slot] >> N.META_LANE_SHIFT) & 0xFF).long()
+            masks.append(available_actions_mask(self._pos[:, slot, 0], self._pos[:, slot, 1], lane, si[:, a], table,
+                                                int(self._params.n_target_speeds)))
+        return torch.stack(masks, dim=1) if self.multi_action else masks[0]
 
     def road_substeps(self, n_substeps: int, action=None) -> None:
         """The reference's operator seam (`AbstractEnv._simulate` without `action_type.act`, abstract.py:304-307):
         `n_substeps` x (`Road.act()`; `Road.step(1 / simulation_frequency)`) on the device state and nothing else — no
         observation, reward, clock or autoreset.  The controlled vehicle acts like `ControlledVehicle.act(None)`; with
-        ContinuousAction, `action` ([N, 2] in [-1, 1]) is the action dict the plain Vehicle keeps (default zeros)."""
+        ContinuousAction, `action` ([N, 2] in [-1, 1]; [N, A, 2] under MultiAgentAction) is the action dict the plain
+        Vehicle keeps (default zeros)."""
         if not self._seeded:
             raise RuntimeError("call reset() before road_substeps()")
         af = None
@@ -311,6 +374,14 @@ class BatchedHighwayEnv(BatchedVectorEnv):
         return sd
 
     def load_state_dict(self, sd: dict, env_ids=None) -> None:
+        """The base fields; with several controlled vehicles every env may hold at most `controlled_vehicles` slots of
+        an MDPVehicle / Vehicle kind (their speed indices are [N, A])."""
+        if self.n_agents > 1:
+            kind = np.asarray(sd["kind"])
+            n_ctrl = ((kind == N.KIND_MDP) | (kind == N.KIND_VEHICLE)).reshape(-1, kind.shape[-1]).sum(axis=1)
+            if (n_ctrl > self.n_agents).any():
+                raise ValueError(f"a state with more than controlled_vehicles = {self.n_agents} controlled vehicles "
+                                 "in an env")
         super().load_state_dict(sd, env_ids)
         if self._traffic is not None and "acceleration_parameters" in sd:
             idx = slice(None) if env_ids is None else torch.from_numpy(np.asarray(env_ids, dtype=np.int64)).to(self.device)
@@ -325,6 +396,13 @@ class BatchedHighwayEnvFast(BatchedHighwayEnv):
 
     ENV_ID = "highway-fast-v0"
     OTHERS_CHECK_COLLISIONS = False
+
+
+def ego_slots(vehicles_count: int, controlled_vehicles: int) -> list:
+    """Slots of the controlled vehicles: near_split(vehicles_count, num_bins=controlled_vehicles) (utils.py:355) gives
+    the quotient, + 1 for the first `remainder` bins, and each bin is one controlled vehicle then its traffic."""
+    q, r = divmod(int(vehicles_count), int(controlled_vehicles))
+    return [k * (q + 1) + min(k, r) for k in range(int(controlled_vehicles))]
 
 
 def available_actions_mask(x, y, lane, speed_index, lane_table, n_speeds: int, vehicle_length: float = 5.0):

@@ -121,7 +121,19 @@ typedef struct HwyHighwayParams {
      * with the default ranges.  Otherwise column c holds feature obs_feature[c] (HWY_FEAT_*), mapped
      * from [obs_feature_lo, obs_feature_hi] to [-1, 1] when obs_normalize and obs_feature_ranged[c]. */
     int32_t obs_n_features;
-    int32_t _pad_obs;
+    /* config["controlled_vehicles"] (0 or 1: one controlled vehicle; at most 8).  With n_agents > 1 the step, reset
+     * and observe entry points run the multi-agent kernels: the controlled vehicles sit at the slots
+     * _create_vehicles gives them (highway_env.py:72-98): bin k of near_split(n_vehicles - n_agents, n_agents)
+     * (utils.py:355) is controlled vehicle k followed by its traffic.  Agent k of a step is the k-th slot whose kind
+     * is HWY_KIND_MDP or HWY_KIND_VEHICLE; speed_index holds [n_envs][n_agents]; reward, flags and info are the
+     * first controlled vehicle's (slot 0).  LinearVehicle traffic is refused with n_agents > 1.
+     *   multi_action (MultiAgentAction, action.py:301-333): action_i [n_envs][n_agents] or action_f
+     *     [n_envs][n_agents][2], one action per controlled vehicle.  0: action_i [n_envs] / action_f [n_envs][2] go
+     *     to the first one and the others act(None): IDLE for an MDPVehicle, the kept {0, 0} for a plain Vehicle.
+     *   multi_obs (MultiAgentObservation, observation.py:588-604): the Kinematics observation is written once per
+     *     controlled vehicle as observer, obs [n_envs][n_agents][K][columns].  0: the first one's, [n_envs][K][..]. */
+    int16_t n_agents;
+    uint8_t multi_action, multi_obs;
     int32_t obs_feature[HWY_MAX_OBS_FEATURES];
     int32_t obs_feature_ranged[HWY_MAX_OBS_FEATURES];
     double obs_feature_lo[HWY_MAX_OBS_FEATURES], obs_feature_hi[HWY_MAX_OBS_FEATURES];
