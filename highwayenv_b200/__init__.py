@@ -28,6 +28,9 @@ REGISTRY = {
     "intersection-v1": "highwayenv_b200.envs.intersection_env:BatchedContinuousIntersectionEnv",
     # ConnectedLaneNeighboursMixin variants (neighbour search across lane segments)
     "roundabout-v1": "highwayenv_b200.envs.roundabout_env:BatchedConnectedLaneRoundaboutEnv",
+    # the roundabout of config["roundabout_radius"] / ["roundabout_lanes"] with vehicles_count rejection-sampled cars
+    "roundabout-generic-v0": "highwayenv_b200.envs.roundabout_env:BatchedRoundaboutGenericEnv",
+    "roundabout-generic-v1": "highwayenv_b200.envs.roundabout_env:BatchedConnectedLaneRoundaboutGenericEnv",
     "intersection-v2": "highwayenv_b200.envs.intersection_env:BatchedConnectedLaneIntersectionEnv",
     "two-way-v0": "highwayenv_b200.envs.two_way_env:BatchedTwoWayEnv",
     "u-turn-v0": "highwayenv_b200.envs.u_turn_env:BatchedUTurnEnv",

@@ -212,6 +212,12 @@ class HwyRoundaboutSpawn(C.Structure):
     ]
 
 
+class HwyRoundaboutGenericSpawn(C.Structure):
+    _fields_ = [("ego_lane", C.c_int32), ("spawn_road", C.c_int32 * 7), ("vehicles_count", C.c_int32),
+                ("fixed_destination", C.c_int32), ("ego_speed_index", C.c_int32), ("route_width", C.c_int32),
+                ("route_table", C.c_void_p), ("route_len", C.c_void_p)]
+
+
 class HwyRacetrackParams(C.Structure):
     _fields_ = [("other_vehicles", C.c_int32), ("terminate_off_road", C.c_int32), ("lane_ab", C.c_int32),
                 ("lane_bc", C.c_int32), ("n_from_nodes", C.c_int32), ("ego_lanes", C.c_int32),
@@ -317,7 +323,7 @@ EXPORTS = (
     "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
     "hwy_lane_keeping_reset", "hwy_lane_keeping_step", "hwy_racetrack_reset", "hwy_racetrack_step",
-    "hwy_debug_network_lanes", "hwy_debug_network_closest_lanes",
+    "hwy_debug_network_lanes", "hwy_debug_network_closest_lanes", "hwy_roundabout_generic_reset",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -389,7 +395,8 @@ def load():
     # the scripted resets: (params, graph, spawn, state, rng, mask_a, mask_b, obs, stream)
     for name, spawn in (("hwy_roundabout_reset", HwyRoundaboutSpawn), ("hwy_merge_reset", HwyMergeSpawn),
                         ("hwy_exit_reset", HwyExitSpawn), ("hwy_u_turn_reset", HwyUTurnSpawn),
-                        ("hwy_two_way_reset", HwyTwoWaySpawn)):
+                        ("hwy_two_way_reset", HwyTwoWaySpawn),
+                        ("hwy_roundabout_generic_reset", HwyRoundaboutGenericSpawn)):
         fn = getattr(lib, name)
         fn.restype = C.c_int
         fn.argtypes = [NP, NG, C.POINTER(spawn), NS] + [C.c_void_p] * 5

@@ -176,7 +176,16 @@ def _connected(base):
     return make
 
 
+def roundabout_generic_default_config() -> dict:
+    """RoundaboutGenericEnv.default_config (highway_env/envs/roundabout_env.py:407-419)."""
+    config = roundabout_default_config()
+    update_config(config, {"roundabout_radius": 20, "roundabout_lanes": 2, "vehicles_count": 5, "duration": 17})
+    return config
+
+
 DEFAULTS["roundabout-v1"] = _connected(roundabout_default_config)
+DEFAULTS["roundabout-generic-v0"] = roundabout_generic_default_config
+DEFAULTS["roundabout-generic-v1"] = _connected(roundabout_generic_default_config)
 DEFAULTS["intersection-v2"] = _connected(intersection_default_config)
 
 

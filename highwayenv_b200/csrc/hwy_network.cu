@@ -2455,6 +2455,99 @@ racetrack_step_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph*
     if (env_ok) store_env(S, st, e, i, i < st.count ? i : -1, r);
 }
 
+// ------------------------------------------------------------------ roundabout-generic-v0 / v1 (envs/roundabout_env.py)
+// RoundaboutGenericEnv._make_vehicles (:664-751), one env per WARP as roundabout_reset_kernel: every lane of the warp
+// walks the env's draw chain redundantly (same instructions, same values), and each placed vehicle's closest-lane search
+// over the table (objects.py:46-50) is spread over the warp, lane l evaluating graph lane l, then a (distance, index)
+// minimum over the warp = np.argmin's first minimum.  The population varies per env: a vehicle whose 10 tries all land
+// within 7 m of a placed point is skipped, S.count receives the population and the slots past it are cleared.
+__global__ void __launch_bounds__(128)
+roundabout_generic_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
+                                const __grid_constant__ HwyRoundaboutGenericSpawn SP,
+                                const __grid_constant__ HwyNetState S, uint64_t* __restrict__ rng,
+                                const uint8_t* __restrict__ mask_a, const uint8_t* __restrict__ mask_b) {
+    const int e = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int wl = threadIdx.x & 31;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;  // warp-uniform
+    Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
+    const size_t base = (size_t)e * S.vp;
+    double xs[HWY_NET_GROUP_LARGE], ys[HWY_NET_GROUP_LARGE];  // spawned_points
+    int n = 0;
+    // make_on_lane (vehicle/objects.py:68-90) into slot n, with plan_route_to(destination) from the closest lane
+    auto place = [&](const HwyNetLane& L, double lon, double px, double py, double speed, double target_speed,
+                     double delta, int dest, int kind) {
+        const double heading = lane_heading_at(L, lon);
+        double bd = INFINITY;
+        int lane = 0x7fffffff;
+        for (int l = wl; l < graph->n_lanes; l += 32) {
+            const double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
+            if (lane == 0x7fffffff || d < bd) {
+                bd = d;
+                lane = l;
+            }
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+            const double d2 = __shfl_xor_sync(0xffffffffu, bd, off);
+            const int l2 = __shfl_xor_sync(0xffffffffu, lane, off);
+            if (l2 != 0x7fffffff && (lane == 0x7fffffff || d2 < bd || (d2 == bd && l2 < lane))) {
+                bd = d2;
+                lane = l2;
+            }
+        }
+        const size_t k = (size_t)lane * SP.route_width + dest;
+        if (wl == 0) {
+            store_vehicle(P, S, base + n, px, py, heading, speed, target_speed, delta, lane, lane, kind);
+            S.route_len[base + n] = SP.route_len[k];
+        }
+        const int* rsrc = SP.route_table + k * R;
+        int* rdst = S.route + (base + n) * R;
+        for (int j = wl; j < R; j += 32) rdst[j] = rsrc[j];
+        xs[n] = px;
+        ys[n] = py;
+        ++n;
+    };
+    {  // :670-685 the ego at the end of ("ser","ses",0), routed to "nxs" (destination 4)
+        const HwyNetLane& L = graph->lanes[SP.ego_lane];
+        const double lon = L.length - 2.5;
+        double px, py;
+        lane_position(L, lon, 0.0, px, py);
+        place(L, lon, px, py, 8.0, P.target_speeds[SP.ego_speed_index], 4.0, 4, HWY_KIND_MDP);
+    }
+    for (int v = 0; v < SP.vehicles_count; ++v) {
+        for (int t = 0; t < 10; ++t) {
+            const int road = SP.spawn_road[g.choice(7)];
+            const HwyNetLane& L = graph->lanes[road + g.choice(graph->lanes[road].road_count)];
+            const double lon = g.uniform(5.0, fmax(5.0, L.length - 5.0));
+            double px, py;
+            lane_position(L, lon, 0.0, px, py);
+            bool safe = true;
+            for (int j = 0; j < n; ++j)
+                if (norm2(px - xs[j], py - ys[j]) < 7.0) {
+                    safe = false;
+                    break;
+                }
+            if (!safe) continue;
+            const double speed = 14.0 + g.normal() * 2.0;
+            const int dest = SP.fixed_destination >= 0 ? SP.fixed_destination : g.choice(4);
+            const double delta = g.uniform(3.5, 4.5);  // randomize_behavior (behavior.py:66-69)
+            place(L, lon, px, py, speed, speed, delta, dest, HWY_KIND_IDM);
+            break;
+        }
+    }
+    for (int v = n + wl; v < S.vp; v += 32) {
+        const size_t k = base + v;
+        reinterpret_cast<double2*>(S.pos)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.hs)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.tt)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.imp)[k] = make_double2(0.0, 0.0);
+        S.delta[k] = 0.0;
+        S.meta[k] = 0;
+        S.route_len[k] = 0;
+    }
+    if (wl == 0) store_env_tail(S, rng, e, SP.ego_speed_index, n, g);
+}
+
 }  // namespace hwynet
 
 // ====================================================================== C ABI
@@ -2857,6 +2950,24 @@ int hwy_roundabout_reset(const HwyNetParams* p, const HwyNetGraph* graph, const 
     if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng pointer");
     if (p->n_vehicles != 5 || s->vp != HWY_NET_GROUP) return fail("%s", "roundabout spawn places exactly 5 vehicles in 8 slots");
     return scripted_reset(hwynet::roundabout_reset_kernel, "roundabout_reset_kernel", 32,  // a warp per env
+                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
+}
+
+int hwy_roundabout_generic_reset(const HwyNetParams* p, const HwyNetGraph* graph,
+                                 const HwyRoundaboutGenericSpawn* spawn, const HwyNetState* s, uint64_t* rng,
+                                 const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
+    if (validate_net(p, graph, s)) return 1;
+    if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng pointer");
+    if (!s->count) return fail("%s", "roundabout-generic: the count buffer receives the population");
+    if (spawn->vehicles_count > s->vp - 1 || p->n_vehicles < 1 + (spawn->vehicles_count > 0 ? spawn->vehicles_count : 0))
+        return fail("%s", "roundabout-generic: vehicles_count exceeds the slots or n_vehicles");
+    if (spawn->fixed_destination < -1 || spawn->fixed_destination > 3 || spawn->route_width < 5)
+        return fail("%s", "roundabout-generic: fixed_destination out of -1..3 or route_width < 5");
+    if (spawn->ego_lane < 0 || spawn->ego_lane >= HWY_NET_MAX_LANES) return fail("%s", "ego_lane out of range");
+    for (int k = 0; k < 7; ++k)
+        if (spawn->spawn_road[k] < 0 || spawn->spawn_road[k] >= HWY_NET_MAX_LANES)
+            return fail("%s", "spawn_road out of range");
+    return scripted_reset(hwynet::roundabout_generic_reset_kernel, "roundabout_generic_reset_kernel", 32,
                           p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 

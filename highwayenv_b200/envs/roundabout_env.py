@@ -14,6 +14,9 @@ order (normal, normal, choice, uniform per traffic vehicle).  Two reset modes:
   in the last ulp (~1e-15 m).  SameStep autoreset stays on the device.
 * ``reset_mode="host"``: the spawn is rebuilt with numpy (bit-identical to the reference) and
   uploaded; autoreset round-trips through the host.
+
+roundabout-generic-v0 / v1 (``RoundaboutGenericEnv``, :398-757) run the same task on a lane table built from the
+config and reset on the device only (``hwy_roundabout_generic_reset``); see ``BatchedRoundaboutGenericEnv``.
 """
 from __future__ import annotations
 
@@ -73,6 +76,89 @@ def make_roundabout_network() -> NetworkTable:
     net.add_straight("wxs", "wxr", [-dev / 2, -2], [-access, -2])
     net.finalize()
     return net
+
+
+GENERIC_MAX_RING_LANES = 2  # 8 arcs per ring lane + 16 access lanes: 3 ring lanes would need 40 of the 32-lane table
+
+
+def make_roundabout_generic_network(radius: float = 20, lanes: int = 2) -> NetworkTable:
+    """RoundaboutGenericEnv._make_road (roundabout_env.py:421-662): `lanes` rings of 8 circular arcs at radii
+    radius + 4 i, then per branch a straight access lane and a sine lane, entries and exits built from the outer
+    ring's points with the reference's float64 expressions, lanes in its insertion order (8 lanes + 16 lanes)."""
+    if not 1 <= lanes <= GENERIC_MAX_RING_LANES:
+        raise ValueError(f"lanes must be in 1..{GENERIC_MAX_RING_LANES}")
+    net = NetworkTable()
+    center, alpha = [0, 0], 24
+    radii = [radius + (4 * i) for i in range(lanes)]
+    n, c, s = 0, 2, 1  # LineType NONE, CONTINUOUS, STRIPED (road/lane.py:12-20)
+    nodes = ["se", "ex", "ee", "nx", "ne", "wx", "we", "sx", "se"]
+    angles = [(90 - alpha, alpha), (alpha, -alpha), (-alpha, -90 + alpha), (-90 + alpha, -90 - alpha),
+              (-90 - alpha, -180 + alpha), (-180 + alpha, -180 - alpha), (180 - alpha, 90 + alpha),
+              (90 + alpha, 90 - alpha)]
+
+    def lane(f, t, line_types, **kw):
+        if "radius" in kw:
+            net.add_circular(f, t, center, kw["radius"], kw["a0"], kw["a1"], clockwise=False)
+        else:
+            net.add_straight(f, t, kw["start"], kw["end"], sine=kw.get("sine"))
+        net._graph[f][t][-1]["line_types"] = list(line_types)
+
+    for k in range(lanes):
+        lt = [c, c] if lanes == 1 else [c, s] if k == 0 else [n, c] if k == lanes - 1 else [n, s]
+        for i in range(8):
+            lane(nodes[i], nodes[i + 1], lt, radius=radii[k], a0=np.deg2rad(angles[i][0]), a1=np.deg2rad(angles[i][1]))
+    outer = radii[-1]
+
+    def pt(angle_deg):
+        rad = np.deg2rad(angle_deg)
+        return [outer * np.cos(rad), outer * np.sin(rad)]
+
+    p_se, p_ex, p_ee, p_nx = pt(90 - alpha), pt(alpha), pt(-alpha), pt(-90 + alpha)
+    p_ne, p_wx, p_we, p_sx = pt(-90 - alpha), pt(-180 + alpha), pt(180 - alpha), pt(90 + alpha)
+    dev = max(100.0, 2 * outer + 40.0)
+    access = dev + 40.0
+    ph = -np.pi / 2
+    # south entry, south exit
+    a, w = (p_se[0] - 2) / 2, np.pi / (dev / 2 - p_se[1])
+    lane("ser", "ses", (s, c), start=[2, access], end=[2, dev / 2])
+    lane("ses", "se", (c, c), start=[2 + a, dev / 2], end=[2 + a, p_se[1]], sine=(a, w, ph))
+    a, w = (p_sx[0] + 2) / 2, np.pi / (dev / 2 - p_sx[1])
+    lane("sx", "sxs", (c, c), start=[p_sx[0] - a, p_sx[1]], end=[p_sx[0] - a, dev / 2], sine=(a, w, ph))
+    lane("sxs", "sxr", (n, c), start=[-2, dev / 2], end=[-2, access])
+    # east entry, east exit
+    a, w = (-2 - p_ee[1]) / 2, np.pi / (dev / 2 - p_ee[0])
+    lane("eer", "ees", (s, c), start=[access, -2], end=[dev / 2, -2])
+    lane("ees", "ee", (c, c), start=[dev / 2, -2 - a], end=[p_ee[0], -2 - a], sine=(a, w, ph))
+    a, w = (2 - p_ex[1]) / 2, np.pi / (dev / 2 - p_ex[0])
+    lane("ex", "exs", (c, c), start=[p_ex[0], p_ex[1] + a], end=[dev / 2, p_ex[1] + a], sine=(a, w, ph))
+    lane("exs", "exr", (n, c), start=[dev / 2, 2], end=[access, 2])
+    # north entry, north exit
+    a, w = (-2 - p_ne[0]) / 2, np.pi / (p_ne[1] - (-dev / 2))
+    lane("ner", "nes", (s, c), start=[-2, -access], end=[-2, -dev / 2])
+    lane("nes", "ne", (c, c), start=[-2 - a, -dev / 2], end=[-2 - a, p_ne[1]], sine=(a, w, ph))
+    a, w = (2 - p_nx[0]) / 2, np.pi / (p_nx[1] - (-dev / 2))
+    lane("nx", "nxs", (c, c), start=[p_nx[0] + a, p_nx[1]], end=[p_nx[0] + a, -dev / 2], sine=(a, w, ph))
+    lane("nxs", "nxr", (n, c), start=[2, -dev / 2], end=[2, -access])
+    # west entry, west exit
+    a, w = (p_we[1] - 2) / 2, np.pi / (p_we[0] - (-dev / 2))
+    lane("wer", "wes", (s, c), start=[-access, 2], end=[-dev / 2, 2])
+    lane("wes", "we", (c, c), start=[-dev / 2, 2 + a], end=[p_we[0], 2 + a], sine=(a, w, ph))
+    a, w = (p_wx[1] + 2) / 2, np.pi / (p_wx[0] - (-dev / 2))
+    lane("wx", "wxs", (c, c), start=[p_wx[0], p_wx[1] - a], end=[-dev / 2, p_wx[1] - a], sine=(a, w, ph))
+    lane("wxs", "wxr", (n, c), start=[-dev / 2, -2], end=[-access, -2])
+    net.finalize()
+    return net
+
+
+_GENERIC_NETS: dict = {}
+
+
+def roundabout_generic_network(radius, lanes) -> NetworkTable:
+    """The lane table of config["roundabout_radius"], config["roundabout_lanes"], cached per pair."""
+    key = (float(radius), int(lanes))
+    if key not in _GENERIC_NETS:
+        _GENERIC_NETS[key] = make_roundabout_generic_network(*key)
+    return _GENERIC_NETS[key]
 
 
 class RoundaboutSpawner:
@@ -291,3 +377,112 @@ class BatchedConnectedLaneRoundaboutEnv(BatchedRoundaboutEnv):
     searches the lane segments connected to the queried lane (road/road.py:509-529)."""
 
     ENV_ID = "roundabout-v1"
+
+
+GENERIC_DESTINATIONS = ["exr", "sxr", "nxr", "wxr"]  # roundabout_env.py:668
+GENERIC_SPAWN_ROADS = [("we", "sx"), ("sx", "se"), ("ee", "nx"), ("nx", "ne"), ("eer", "ees"), ("ner", "nes"),
+                       ("wer", "wes")]  # :690-698
+
+
+def check_roundabout_generic(cfg: dict, env_id: str) -> None:
+    """The generic roundabout's own keys: raises for what the reference cannot build or the kernels cannot hold."""
+    lanes, radius, count = cfg["roundabout_lanes"], cfg["roundabout_radius"], cfg["vehicles_count"]
+    if isinstance(lanes, bool) or int(lanes) != lanes:
+        raise ValueError("roundabout_lanes must be an integer")
+    if lanes < 1:
+        raise ValueError("roundabout_lanes must be >= 1 (the reference raises IndexError on an empty ring)")
+    if lanes > GENERIC_MAX_RING_LANES:
+        raise NotImplementedError(f"roundabout_lanes > {GENERIC_MAX_RING_LANES} on {env_id}: {8 * lanes + 16} lanes "
+                                  f"exceed the {N.HWY_NET_MAX_LANES}-lane table")
+    if isinstance(radius, bool) or not np.isfinite(float(radius)) or radius <= 0:
+        raise ValueError("roundabout_radius must be a positive number")
+    if isinstance(count, bool) or int(count) != count:
+        raise ValueError("vehicles_count must be an integer")
+    if count > N.HWY_NET_GROUP_LARGE - 1:
+        raise NotImplementedError(f"vehicles_count > {N.HWY_NET_GROUP_LARGE - 1} on {env_id}: the ego and its traffic "
+                                  f"fill at most {N.HWY_NET_GROUP_LARGE} slots")
+    fd = cfg["incoming_vehicle_destination"]
+    if fd is not None and int(fd) < -len(GENERIC_DESTINATIONS):
+        raise IndexError("list index out of range")  # destinations[min(d, 3)] in the reference
+
+
+class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
+    """`roundabout-generic-v0`: RoundaboutGenericEnv (roundabout_env.py:398-751), RoundaboutEnv's rewards, termination
+    and dynamics on a roundabout of config["roundabout_lanes"] ring lanes (1..2) at config["roundabout_radius"], with
+    config["vehicles_count"] traffic vehicles placed by rejection sampling (``hwy_roundabout_generic_reset``).  A
+    vehicle whose 10 tries fail is skipped, so the population varies per env (``count``).  Up to 7 traffic vehicles
+    run on 8 slots (``hwy_network_step``), 8 to 31 on 32 slots (``hwy_intersection_step`` without rules or spawns).
+    The lane table follows the config: reset(options={"config": ...}) rebuilds it and re-allocates."""
+
+    ENV_ID = "roundabout-generic-v0"
+    RESET_ENTRY = "hwy_roundabout_generic_reset"
+
+    def _make_network(self) -> NetworkTable:
+        return self._road
+
+    def define_spaces(self) -> None:
+        if self.reset_mode != "device":
+            raise NotImplementedError(f"{self.ENV_ID} resets on the device ({self.RESET_ENTRY})")
+        cfg = self.config
+        check_roundabout_generic(cfg, self.ENV_ID)
+        road = roundabout_generic_network(cfg["roundabout_radius"], cfg["roundabout_lanes"])
+        if self._net is not road:  # another (radius, lanes): rebuild the device table
+            self._net = None
+        self._road = road
+        count = int(cfg["vehicles_count"])
+        self.N_VEHICLES = 1 + max(count, 0)
+        self.SLOTS = N.HWY_NET_GROUP if self.N_VEHICLES <= N.HWY_NET_GROUP else N.HWY_NET_GROUP_LARGE
+        super().define_spaces()
+
+    def _allocate(self) -> None:
+        super()._allocate()  # the 32-slot state already carries the population and the (unused) rule clock
+        if self.vp == N.HWY_NET_GROUP:  # the 8-slot kernels read the population when the state carries one
+            self._count = torch.full((self.num_envs,), self.N_VEHICLES, dtype=torch.int32, device=self.device)
+            self._state.count = self._count.data_ptr()
+            self._road_steps = None
+
+    def _build_spawn_tables(self) -> None:
+        net, cfg = self.net, self.config
+        table, _ = self._route_tables(GENERIC_DESTINATIONS + ["nxs"])
+        s = N.HwyRoundaboutGenericSpawn()
+        s.ego_lane = net.index[("ser", "ses", 0)]
+        for k, (f, t) in enumerate(GENERIC_SPAWN_ROADS):
+            s.spawn_road[k] = net.index[(f, t, 0)]
+        s.vehicles_count = int(cfg["vehicles_count"])
+        fd = cfg["incoming_vehicle_destination"]
+        s.fixed_destination = -1 if fd is None else min(int(fd), 3) % len(GENERIC_DESTINATIONS)
+        s.ego_speed_index = speed_to_index(self.action_type.target_speeds, 8.0)
+        s.route_width = table.shape[1]
+        s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
+        self._spawn_struct = s
+
+    def to_finite_mdp(self):
+        raise NotImplementedError(f"to_finite_mdp on {self.ENV_ID}")
+
+    def copy_envs(self, dst_ids, src_ids, source=None) -> None:
+        """BatchedVectorEnv.copy_envs; two envs of one class may still run different lane tables (radius, lanes) or
+        slot strides, and a state only means something on its own table."""
+        if source is not None and type(source) is type(self) and (source._road is not self._road
+                                                                   or source.vp != self.vp):
+            raise ValueError(f"copy_envs between {self.ENV_ID} envs on different roads (roundabout_radius, "
+                             "roundabout_lanes) or slot strides")
+        super().copy_envs(dst_ids, src_ids, source)
+
+    def state_dict(self) -> dict:
+        """RoundaboutEnv's fields [N, V] with V = 1 + vehicles_count; `count` vehicles of each env are on the road."""
+        sd = super().state_dict()
+        sd["count"] = self._count.cpu().numpy()
+        return sd
+
+    def load_state_dict(self, sd: dict, env_ids=None) -> None:
+        super().load_state_dict(sd, env_ids)
+        idx = slice(None) if env_ids is None else torch.from_numpy(np.asarray(env_ids, dtype=np.int64)).to(self.device)
+        self._count[idx] = torch.from_numpy(np.asarray(sd["count"], dtype=np.int32).reshape(-1)).to(self.device)
+        if self._road_steps is not None:
+            self._road_steps[idx] = 0
+
+
+class BatchedConnectedLaneRoundaboutGenericEnv(BatchedRoundaboutGenericEnv):
+    """`roundabout-generic-v1`: ConnectedLaneNeighboursMixin over the generic roundabout."""
+
+    ENV_ID = "roundabout-generic-v1"

@@ -549,6 +549,30 @@ int hwy_roundabout_reset(const HwyNetParams *p, const HwyNetGraph *graph, const 
                          const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
                          float *obs, void *stream);
 
+/* RoundaboutGenericEnv._make_vehicles (envs/roundabout_env.py:664-751; roundabout-generic-v0 / v1) on the device:
+ * the MDPVehicle at length - 2.5 of ("ser","ses",0), speed 8, routed to "nxs"; then for each of vehicles_count
+ * vehicles up to 10 tries of integers(0, 7) (spawn road), integers(0, lanes of the road) (no draw on a one-lane
+ * road), uniform(5, max(5, length - 5)) (longitudinal), rejected when the point lies closer than 7 m to a point
+ * already placed; an accepted try draws its speed 14 + 2 normal(), its destination integers(0, 4) (none when
+ * fixed_destination >= 0) and DELTA uniform(3.5, 4.5), and plans its route from its closest lane.  A vehicle whose
+ * 10 tries all fail is skipped: s->count (required) receives the population and the slots past it are cleared.
+ * Slot stride 8 or 32. */
+typedef struct HwyRoundaboutGenericSpawn {
+    int32_t ego_lane;            /* table index of ("ser", "ses", 0) */
+    int32_t spawn_road[7];       /* table index of lane 0 of (we,sx), (sx,se), (ee,nx), (nx,ne), (eer,ees), (ner,nes),
+                                  * (wer,wes) */
+    int32_t vehicles_count;      /* config["vehicles_count"], at most s->vp - 1 (<= 0: the ego alone) */
+    int32_t fixed_destination;   /* destinations[min(incoming_vehicle_destination, 3)] as 0..3; -1 = None (drawn) */
+    int32_t ego_speed_index;     /* MDPVehicle.speed_to_index(8) */
+    int32_t route_width;         /* destinations per lane of the route table, >= 5 */
+    const int32_t *route_table;  /* DEVICE [n_lanes][route_width][HWY_NET_MAX_ROUTE]; destination 0..3 = exr, sxr,
+                                  * nxr, wxr; 4 = the ego's nxs */
+    const int32_t *route_len;    /* DEVICE [n_lanes][route_width] */
+} HwyRoundaboutGenericSpawn;
+int hwy_roundabout_generic_reset(const HwyNetParams *p, const HwyNetGraph *graph,
+                                 const HwyRoundaboutGenericSpawn *spawn, const HwyNetState *s, uint64_t *rng,
+                                 const uint8_t *mask_a, const uint8_t *mask_b, float *obs, void *stream);
+
 /* RacetrackEnv (envs/racetrack_env.py:15-425; racetrack-v0, and racetrack-v1 with connected_lanes) and its large
  * (RacetrackEnvLarge, :432-880) and oval (RacetrackEnvOval, :882-1396) tracks on the 8-slot network state, which must carry s->count (the population: the ego, the front vehicle and the extra vehicles that
  * survived the 20 m check).  The controlled vehicle is a plain Vehicle (HWY_KIND_VEHICLE) in slot 0 whose (target_speed,
