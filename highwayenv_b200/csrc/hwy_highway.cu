@@ -37,8 +37,12 @@ namespace hwy {
 
 // Optional per-phase cycle accounting (-DHWY_PHASE_TIMING): warp-level clock64() deltas summed
 // into g_phase_cycles; read with hwy_debug_phase_cycles().  Off in the shipped build.
+// The same build counts how the road order of each env-frame was found (g_order_probe, hwy_debug_order_probe()):
+// [0] env-frames, [1] those whose previous order failed the chain check, [2] envs that ran rank_count, [3] warp
+// cycles spent recovering a failed order (summed over the warps that did).
 #ifdef HWY_PHASE_TIMING
 __device__ unsigned long long g_phase_cycles[16];
+__device__ unsigned long long g_order_probe[4];
 #define PHASE_INIT() long long _pt = clock64()
 #define PHASE_MARK(k)                                                                 \
     do {                                                                              \
@@ -63,9 +67,15 @@ struct Frame {
     uint32_t lane_is[HWY_MAX_LANES][NW];     // vehicles whose lane_index is l    (slot order)
     uint32_t fired[NW];                      // IDM vehicles whose lane-change timer will fire
     unsigned char lane[TPE], tgt[TPE], perm[TPE], rank[TPE];
+    unsigned char on_lanes[TPE];             // kWarpOrder: bit l = on_lane(margin=1) of lane l, by slot
     int slow;                                // ties in ls or unaligned lanes: use the linear scans
     unsigned vmax_bits;                      // max(0, max speed) of the env, float bits rounded up (pruned sweep bound)
 };
+
+// Dense env segments of 33 to 64 vehicles: one warp per env finds the road order (warp_order) and builds the
+// rank-ordered membership masks; every other step kernel counts ranks per vehicle (build_frame).
+template <int TPE, bool DENSE>
+constexpr bool kWarpOrder = DENSE && TPE == 64;
 
 template <int TPE>
 struct EnvShared {
@@ -513,9 +523,10 @@ __device__ __forceinline__ void stage_stored_order(Frame<TPE>& G, int i, int V, 
 
 // Stage one vehicle into frame F (plain stores) and clear the words of F that build_frame fills
 // with atomics (DENSE: the caller does, clear_masks).  Callers put a barrier between publish() and build_frame().
+// lane_bits (kWarpOrder kernels, frames that act): the vehicle's on_lane(margin=1) bits for warp_order's masks.
 template <int TPE, bool LINEAR = false, bool DENSE = false>
 __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F, int i, bool active,
-                                        const VehicleRegs& r) {
+                                        const VehicleRegs& r, bool lane_bits = false) {
     constexpr int NW = TPE / 32;
     if (active) {
         double sn, cs;
@@ -529,9 +540,19 @@ __device__ __forceinline__ void publish(const HwyHighwayParams& P, Frame<TPE>& F
         // default is the vehicle's own speed (behavior.py:449-452)
         F.ts[i] = meta_kind(r.meta) == HWY_KIND_VEHICLE ? (LINEAR ? r.speed : 0.0) : r.target_speed;
         F.ls[i] = lane_s(P.lanes[0], r.x, r.y);
-        F.lsf[i] = (float)F.ls[i];
+        if constexpr (!kWarpOrder<TPE, DENSE>) F.lsf[i] = (float)F.ls[i];
         F.lane[i] = (unsigned char)meta_lane(r.meta);
         F.tgt[i] = (unsigned char)meta_target(r.meta);
+        if (lane_bits) {
+            unsigned bits = 0;
+#pragma unroll 1
+            for (int l = 0; l < P.lanes_count; ++l) {
+                double s_l, lat_l;
+                lane_local(P.lanes[l], r.x, r.y, s_l, lat_l);
+                if (lane_on(P.lanes[l], s_l, lat_l, 1.0)) bits |= 1u << l;
+            }
+            F.on_lanes[i] = (unsigned char)bits;
+        }
     }
     if (!DENSE && i < HWY_MAX_LANES * NW) (&F.smask[0][0])[i] = 0;
     if (i == 0) {
@@ -731,6 +752,98 @@ __device__ __noinline__ int rank_repair(const Frame<TPE>& F, const Frame<TPE>& p
     return r0;
 }
 
+// kWarpOrder kernels: the road order of one env by one warp, after the barrier that follows publish().  The reference's
+// order is the rank of (s, slot): s ascending, equal s by slot, which rank_count computes too.  The warp sorts the
+// previous frame's permutation by that key, lane L holding positions 2L and 2L + 1 (V <= 64, the positions past V
+// +inf sentinels), with odd-even transposition passes (an in-lane and a cross-lane compare-exchange each) until a
+// pass swaps nothing.  A pass that swaps nothing is the chain check, one overtake costs one more pass, and 32 passes
+// sort any order of 64 entries.  The first frame's stored order need not be a permutation (stale or repeated
+// entries): it is checked with two reductions and replaced by the identity if it is not one.  The warp
+// writes perm, rank, F.slow on equal s (the tie rules of the exact scan) and, when `lanes` > 0, the rank-ordered
+// membership masks from publish()'s on_lanes bits.  Out of line: a block runs it once per env and frame.
+template <int TPE>
+__device__ __noinline__ void warp_order(Frame<TPE>& F, const Frame<TPE>& prev, int V, int lanes) {
+    static_assert(TPE == 64, "two positions per lane");
+    const int L = lane_id(), k0 = 2 * L, k1 = 2 * L + 1;
+    int u0 = k0 < V ? prev.perm[k0] : k0, u1 = k1 < V ? prev.perm[k1] : k1;
+    {
+        uint32_t lo = 0, hi = 0;
+        if (k0 < V) (u0 < 32 ? lo : hi) |= 1u << (u0 & 31);
+        if (k1 < V) (u1 < 32 ? lo : hi) |= 1u << (u1 & 31);
+        lo = __reduce_or_sync(0xffffffffu, lo);
+        hi = __reduce_or_sync(0xffffffffu, hi);
+        const bool perm = lo == (V >= 32 ? ~0u : (1u << V) - 1u) && hi == (V > 32 ? ~0u >> (64 - V) : 0u);
+        if (!perm) {
+            u0 = k0;
+            u1 = k1;
+        }
+    }
+    double d0 = k0 < V ? F.ls[u0] : (double)INFINITY, d1 = k1 < V ? F.ls[u1] : (double)INFINITY;
+    auto after = [](double da, int ua, double db, int ub) { return da > db || (da == db && ua > ub); };
+#ifdef HWY_PHASE_TIMING
+    const long long t_order = clock64();
+#endif
+    bool tie = false;
+    int pass = 0;
+#pragma unroll 1
+    for (;; ++pass) {
+        const bool sw = after(d0, u0, d1, u1);
+        tie = k1 < V && d0 == d1;
+        if (sw) {
+            const double d = d0;
+            d0 = d1;
+            d1 = d;
+            const int u = u0;
+            u0 = u1;
+            u1 = u;
+        }
+        const double dn = __shfl_down_sync(0xffffffffu, d0, 1), dp = __shfl_up_sync(0xffffffffu, d1, 1);
+        const int un = __shfl_down_sync(0xffffffffu, u0, 1), up = __shfl_up_sync(0xffffffffu, u1, 1);
+        const bool sw_hi = L < 31 && after(d1, u1, dn, un);  // positions 2L + 1, 2L + 2
+        const bool sw_lo = L > 0 && after(dp, up, d0, u0);   // positions 2L - 1, 2L (lane L - 1's sw_hi)
+        tie = tie || (k1 + 1 < V && d1 == dn);
+        if (sw_hi) {
+            d1 = dn;
+            u1 = un;
+        }
+        if (sw_lo) {
+            d0 = dp;
+            u0 = up;
+        }
+        if (!__any_sync(0xffffffffu, sw || sw_hi) || pass == 32) break;
+    }
+#ifdef HWY_PHASE_TIMING
+    if (L == 0) {
+        atomicAdd(&g_order_probe[0], 1ull);
+        if (pass > 0) {
+            atomicAdd(&g_order_probe[1], 1ull);
+            atomicAdd(&g_order_probe[3], (unsigned long long)(clock64() - t_order));
+        }
+    }
+#endif
+    if (k0 < V) {
+        F.perm[k0] = (unsigned char)u0;
+        F.rank[u0] = (unsigned char)k0;
+    }
+    if (k1 < V) {
+        F.perm[k1] = (unsigned char)u1;
+        F.rank[u1] = (unsigned char)k1;
+    }
+    if (__any_sync(0xffffffffu, tie) && L == 0) F.slow = 1;
+    if (lanes == 0) return;
+    const unsigned b0 = k0 < V ? F.on_lanes[u0] : 0u, b1 = k1 < V ? F.on_lanes[u1] : 0u;
+#pragma unroll 1
+    for (int l = 0; l < lanes; ++l) {
+        const uint32_t two = (((b0 >> l) & 1u) | (((b1 >> l) & 1u) << 1)) << (2 * (L & 15));
+        const uint32_t lo = __reduce_or_sync(0xffffffffu, L < 16 ? two : 0u);
+        const uint32_t hi = __reduce_or_sync(0xffffffffu, L < 16 ? 0u : two);
+        if (L == 0) {
+            F.smask[l][0] = lo;
+            F.smask[l][1] = hi;
+        }
+    }
+}
+
 // After a barrier that follows publish(): ranks, rank-ordered membership masks, lane / target
 // masks (warp ballots) and the first pass of the collision sweep of Road.step
 // (road/road.py:477-481).  All threads of the env call this convergently.
@@ -755,7 +868,9 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     // swapped or drew level.  The chain also proves that the V entries are V distinct vehicles, so the stored order
     // needs no other check: whatever it came from, a permutation that orders the current keys strictly is their order.
     bool reuse = false;
-    if constexpr (!DENSE) {
+    if constexpr (kWarpOrder<TPE, DENSE>) {
+        // warp_order found the order and the masks; the vehicles read their rank after the next barrier
+    } else if constexpr (!DENSE) {
         bool ok = true;
 #pragma unroll 1
         for (int k = (i & 31) + 1; k < V; k += 32) ok = ok && (F.lsf[prev.perm[k - 1]] < F.lsf[prev.perm[k]]);
@@ -777,7 +892,9 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
         }
     }
     bool tie = false;
-    if constexpr (!DENSE) {
+    if constexpr (kWarpOrder<TPE, DENSE>) {
+        if (active && !aligned) F.slow = 1;
+    } else if constexpr (!DENSE) {
         if (reuse) {
             rank = active ? prev.rank[i] : 0;
         } else {
@@ -789,8 +906,14 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
         }
     } else {
         // the verdict differs between the segments of a warp, and the repair is warp-wide
+#ifdef HWY_PHASE_TIMING
+        const long long t_order = clock64();
+#endif
         int rt = -1;
         if (TPE >= 128 && __any_sync(0xffffffffu, !reuse)) rt = rank_repair<TPE, DENSE>(F, prev, V, i, active);
+#ifdef HWY_PHASE_TIMING
+        const bool repaired = rt >= 0;
+#endif
         if (reuse) {
             rank = active ? prev.rank[i] : 0;
         } else if (active) {
@@ -798,15 +921,26 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
             rank = rt & 0xff;
             tie = (rt >> 8) != 0;
         }
+#ifdef HWY_PHASE_TIMING
+        __syncwarp();
+        const long long t_end = clock64();
+        if (__any_sync(0xffffffffu, active && !reuse) && lane_id() == 0)
+            atomicAdd(&g_order_probe[3], (unsigned long long)(t_end - t_order));
+        if (active && i == 0) {
+            atomicAdd(&g_order_probe[0], 1ull);
+            if (!reuse) atomicAdd(&g_order_probe[1], 1ull);
+            if (!reuse && !repaired) atomicAdd(&g_order_probe[2], 1ull);
+        }
+#endif
     }
-    if (active) {
+    if (!kWarpOrder<TPE, DENSE> && active) {
         F.perm[rank] = (unsigned char)i;
         F.rank[i] = (unsigned char)rank;
         if (tie || !aligned) F.slow = 1;
     }
     // -- the membership masks serve Road.act only, which the last frame of a launch does not run (do_masks, uniform)
     if (do_masks) {
-        if (active) {
+        if (!kWarpOrder<TPE, DENSE> && active) {
 #pragma unroll 1
             for (int l = 0; l < P.lanes_count; ++l) {
                 double s_l, lat_l;
@@ -1897,6 +2031,19 @@ int hwy_debug_phase_cycles(unsigned long long* out16) {
     return 0;
 #else
     for (int k = 0; k < 16; ++k) out16[k] = 0;
+    return 0;
+#endif
+}
+
+// debug: read and clear the road-order counters (all zero unless built with HWY_PHASE_TIMING)
+int hwy_debug_order_probe(unsigned long long* out4) {
+#ifdef HWY_PHASE_TIMING
+    unsigned long long zero[4] = {0};
+    if (cudaMemcpyFromSymbol(out4, hwy::g_order_probe, sizeof(zero)) != cudaSuccess) return 1;
+    if (cudaMemcpyToSymbol(hwy::g_order_probe, zero, sizeof(zero)) != cudaSuccess) return 1;
+    return 0;
+#else
+    for (int k = 0; k < 4; ++k) out4[k] = 0;
     return 0;
 #endif
 }

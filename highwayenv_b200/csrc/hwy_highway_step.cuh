@@ -102,14 +102,18 @@
     for (int frame = 0;; ++frame) {
         p ^= 1;
         Frame<TPE>& F = sm.f[p];
-        publish<TPE, LINEAR, DENSE>(P, F, i, active, r);
         const bool acts = frame < frames;  // the last frame only feeds the collision sweep and the epilogue
+        publish<TPE, LINEAR, DENSE>(P, F, i, active, r, kWarpOrder<TPE, DENSE> && acts);
         if (DENSE && active && acts) clear_masks(F, i, V);
         PHASE_MARK(1);  // publish
         env_sync<TPE>();
         PHASE_MARK(2);  // barrier after publish
         if (i < NW) sm.mid[i] = sm.ok_left[i] = sm.ok_right[i] = 0;  // all readers are past phase B
         if (i == 0) sm.n_items = 0;
+        // warp w finds the road order of env w (a dense block has more warps than envs: V > 32)
+        if constexpr (kWarpOrder<TPE, DENSE>)
+            if ((int)(threadIdx.x >> 5) < EPB)
+                warp_order(smem[threadIdx.x >> 5].f[p], smem[threadIdx.x >> 5].f[p ^ 1], V, acts ? P.lanes_count : 0);
         // frame 0: masks only — the sweep of the stored state ran at the end of the substep that
         // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).  The last frame: ranks and
         // the sweep, no masks.
