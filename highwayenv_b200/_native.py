@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("HWYB200_LIB") or os.path.join(_HERE, "csrc", "libhwyb200.so")
 
-HWY_ABI_VERSION = 16 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
+HWY_ABI_VERSION = 17 # bump with every change of a struct or signature: a stale libhwyb200.so then fails to load
 HWY_MAX_LANES = 8
 HWY_MAX_TARGET_SPEEDS = 8
 HWY_MAX_VEHICLES = 128
@@ -225,6 +225,21 @@ class HwyRacetrackParams(C.Structure):
                 ("action_reward", C.c_double), ("collision_reward", C.c_double), ("on_road_reward", C.c_double)]
 
 
+# HwyNetScenario.kind: the union member the network reset / step / substeps entry points read
+(HWY_SCENARIO_NONE, HWY_SCENARIO_ROUNDABOUT, HWY_SCENARIO_ROUNDABOUT_GENERIC, HWY_SCENARIO_MERGE, HWY_SCENARIO_TWO_WAY,
+ HWY_SCENARIO_U_TURN, HWY_SCENARIO_EXIT, HWY_SCENARIO_INTERSECTION, HWY_SCENARIO_RACETRACK) = range(9)
+
+
+class HwyNetScenarioUnion(C.Union):
+    _fields_ = [("roundabout", HwyRoundaboutSpawn), ("roundabout_generic", HwyRoundaboutGenericSpawn),
+                ("merge", HwyMergeSpawn), ("two_way", HwyTwoWaySpawn), ("u_turn", HwyUTurnSpawn), ("exit", HwyExitSpawn),
+                ("intersection", HwyIntersectionSpawn), ("racetrack", HwyRacetrackParams)]
+
+
+class HwyNetScenario(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("_pad", C.c_int32), ("u", HwyNetScenarioUnion)]
+
+
 FEAT_ON_ROAD, FEAT_UNKNOWN = 13, 14
 HWY_NET_MAX_ROUTE = 16
 
@@ -313,17 +328,16 @@ class HwyLaneKeepingState(C.Structure):
 
 
 EXPORTS = (
-    "hwy_observe_grid", "hwy_observe_ttc", "hwy_observe_lidar", "hwy_exit_reset",
+    "hwy_observe_grid", "hwy_observe_ttc", "hwy_observe_lidar",
     "hwy_abi_version", "hwy_last_error", "hwy_highway_slot_stride", "hwy_highway_reset",
     "hwy_highway_observe", "hwy_highway_step", "hwy_highway_substeps", "hwy_launch_count",
-    "hwy_network_obs_size", "hwy_network_step", "hwy_network_observe", "hwy_roundabout_reset",
-    "hwy_intersection_step", "hwy_network_substeps", "hwy_intersection_reset",
-    "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect", "hwy_merge_reset",
-    "hwy_two_way_reset", "hwy_u_turn_reset", "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
+    "hwy_network_obs_size", "hwy_network_reset", "hwy_network_step", "hwy_network_substeps", "hwy_network_observe",
+    "hwy_debug_network_neighbours", "hwy_debug_rotated_rectangles_intersect",
+    "hwy_debug_math", "hwy_debug_pcg64", "hwy_finite_mdp",
     "hwy_value_iteration", "hwy_copy_env_rows", "hwy_available_actions", "hwy_opd_select", "hwy_opd_record",
     "hwy_opd_recommend", "hwy_mcts_advance", "hwy_mcts_backup", "hwy_mcts_recommend", "hwy_mcts_reroot",
-    "hwy_lane_keeping_reset", "hwy_lane_keeping_step", "hwy_racetrack_reset", "hwy_racetrack_step",
-    "hwy_debug_network_lanes", "hwy_debug_network_closest_lanes", "hwy_roundabout_generic_reset",
+    "hwy_lane_keeping_reset", "hwy_lane_keeping_step",
+    "hwy_debug_network_lanes", "hwy_debug_network_closest_lanes",
 )
 
 # hwy_debug_math ops and their operand / result counts per input (include/hwyb200.h)
@@ -369,16 +383,18 @@ def load():
                                      C.c_void_p, C.c_void_p]
     lib.hwy_highway_substeps.restype = C.c_int
     lib.hwy_highway_substeps.argtypes = [P, S, T, C.c_int, C.c_void_p, C.c_void_p]
-    NP, NG, NS = C.POINTER(HwyNetParams), C.c_void_p, C.POINTER(HwyNetState)
+    # the network reset / step / substeps take the scenario SC (None: kind NONE, except for the reset)
+    NP, NG, NS, SC = C.POINTER(HwyNetParams), C.c_void_p, C.POINTER(HwyNetState), C.POINTER(HwyNetScenario)
     lib.hwy_network_obs_size.restype = C.c_int
     lib.hwy_network_obs_size.argtypes = [NP]
+    lib.hwy_network_reset.restype = C.c_int
+    lib.hwy_network_reset.argtypes = [NP, NG, SC, NS] + [C.c_void_p] * 5
     lib.hwy_network_step.restype = C.c_int
-    lib.hwy_network_step.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                     C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hwy_network_step.argtypes = [NP, NG, SC, NS] + [C.c_void_p] * 10
+    lib.hwy_network_substeps.restype = C.c_int
+    lib.hwy_network_substeps.argtypes = [NP, NG, SC, NS, C.c_void_p, C.c_int, C.c_void_p]
     lib.hwy_network_observe.restype = C.c_int
     lib.hwy_network_observe.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p]
-    lib.hwy_intersection_step.restype = C.c_int
-    lib.hwy_intersection_step.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS] + [C.c_void_p] * 10
     lib.hwy_debug_network_neighbours.restype = C.c_int
     lib.hwy_debug_network_neighbours.argtypes = [NP, NG, NS, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.hwy_debug_network_closest_lanes.restype = C.c_int
@@ -392,19 +408,6 @@ def load():
     lib.hwy_debug_pcg64.restype = C.c_int
     lib.hwy_debug_pcg64.argtypes = [C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_int, C.c_void_p]
-    # the scripted resets: (params, graph, spawn, state, rng, mask_a, mask_b, obs, stream)
-    for name, spawn in (("hwy_roundabout_reset", HwyRoundaboutSpawn), ("hwy_merge_reset", HwyMergeSpawn),
-                        ("hwy_exit_reset", HwyExitSpawn), ("hwy_u_turn_reset", HwyUTurnSpawn),
-                        ("hwy_two_way_reset", HwyTwoWaySpawn),
-                        ("hwy_roundabout_generic_reset", HwyRoundaboutGenericSpawn)):
-        fn = getattr(lib, name)
-        fn.restype = C.c_int
-        fn.argtypes = [NP, NG, C.POINTER(spawn), NS] + [C.c_void_p] * 5
-    lib.hwy_intersection_reset.restype = C.c_int
-    lib.hwy_intersection_reset.argtypes = [NP, NG, C.POINTER(HwyIntersectionSpawn), NS, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.hwy_network_substeps.restype = C.c_int
-    lib.hwy_network_substeps.argtypes = [NP, NG, NS, C.c_void_p, C.c_int, C.c_void_p]
     OV = C.POINTER(HwyObsView)
     lib.hwy_observe_grid.restype = C.c_int
     lib.hwy_observe_grid.argtypes = [NG, OV, C.POINTER(HwyGridParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -441,11 +444,6 @@ def load():
     lib.hwy_lane_keeping_reset.argtypes = [LP, LS] + [C.c_void_p] * 4
     lib.hwy_lane_keeping_step.restype = C.c_int
     lib.hwy_lane_keeping_step.argtypes = [LP, LS] + [C.c_void_p] * 7
-    RP = C.POINTER(HwyRacetrackParams)
-    lib.hwy_racetrack_reset.restype = C.c_int
-    lib.hwy_racetrack_reset.argtypes = [NP, NG, RP, NS] + [C.c_void_p] * 5
-    lib.hwy_racetrack_step.restype = C.c_int
-    lib.hwy_racetrack_step.argtypes = [NP, NG, RP, NS, C.c_void_p, C.c_int] + [C.c_void_p] * 7
     if lib.hwy_abi_version() != HWY_ABI_VERSION:
         raise RuntimeError("libhwyb200.so ABI version mismatch; rebuild")
     _lib = lib

@@ -2726,20 +2726,39 @@ int launch_intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, c
     return check_launch("intersection_reset_kernel");
 }
 
+// The SameStep autoreset's info["final_obs"]: obs as it was before the reset rewrites it
+void keep_final_obs(const HwyNetParams* p, const HwyNetState* s, const float* obs, float* final_obs, cudaStream_t st) {
+    if (final_obs)
+        cudaMemcpyAsync(final_obs, obs, (size_t)s->n_envs * hwy_network_obs_size(p) * sizeof(float),
+                        cudaMemcpyDeviceToDevice, st);
+}
+
+int intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
+                       const HwyNetState* s, const uint8_t* mask_a, const uint8_t* mask_b, float* obs, float* final_obs,
+                       cudaStream_t st) {
+    cudaMemsetAsync(spawn->scratch, 0, sizeof(int), st);
+    hwynet::compact_envs_kernel<<<(s->n_envs + 255) / 256, 256, 0, st>>>(mask_a, mask_b, s->n_envs, spawn->scratch);
+    keep_final_obs(p, s, obs, final_obs, st);
+    if (check_launch("compact_envs_kernel")) return 1;
+    if (spawn->initial_vehicle_count + 1 <= 16)  // n-1 draws + challenger + controlled vehicle fit 16 slots
+        return launch_intersection_reset<16>(p, graph, spawn, s, obs, st);
+    return launch_intersection_reset<HWY_NET_GROUP_LARGE>(p, graph, spawn, s, obs, st);
+}
+
 // A scripted reset: the family kernel over 128-thread blocks, `threads_per_env` (1, or 32 for roundabout) per env,
 // then the fresh observation of the envs it reset
 template <typename K, typename Spawn>
 int scripted_reset(K kernel, const char* name, int threads_per_env, const HwyNetParams* p, const HwyNetGraph* graph,
-                   const Spawn* spawn, const HwyNetState* s, uint64_t* rng, const uint8_t* mask_a,
-                   const uint8_t* mask_b, float* obs, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
+                   const Spawn& spawn, const HwyNetState* s, const uint8_t* mask_a, const uint8_t* mask_b, float* obs,
+                   float* final_obs, cudaStream_t st) {
+    keep_final_obs(p, s, obs, final_obs, st);
     const int per = 128 / threads_per_env;
-    kernel<<<(s->n_envs + per - 1) / per, 128, 0, st>>>(*p, graph, *spawn, *s, rng, mask_a, mask_b);
+    kernel<<<(s->n_envs + per - 1) / per, 128, 0, st>>>(*p, graph, spawn, *s, s->rng, mask_a, mask_b);
     if (check_launch(name)) return 1;
     return obs ? observe_dispatch(p, graph, s, mask_a, mask_b, obs, st) : 0;
 }
+
 int validate_racetrack(const HwyNetParams* p, const HwyRacetrackParams* rp, const HwyNetState* s) {
-    if (!rp) return fail("%s", "null racetrack params");
     if (s->vp != HWY_NET_GROUP || !s->count) return fail("%s", "racetrack: slot stride 8 and the count buffer");
     if (rp->other_vehicles < 0 || rp->other_vehicles > HWY_NET_GROUP - 1)
         return fail("%s", "racetrack: other_vehicles out of range (0..7)");
@@ -2753,42 +2772,30 @@ int validate_racetrack(const HwyNetParams* p, const HwyRacetrackParams* rp, cons
     return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int hwy_network_obs_size(const HwyNetParams* p) {
-    if (!p) return 0;
-    const int agents = p->n_agents > 1 ? p->n_agents : 1;  // one observation per controlled vehicle
-    if (p->obs_type == HWY_OBS_OCCUPANCY) return agents * 4 * 11 * 11;
-    if (p->obs_type == HWY_OBS_TTC) return agents * 9 * (int)(p->ttc_horizon / (1.0 / p->policy_frequency));
-    return agents * p->obs_vehicles_count * (p->obs_n_feat > 0 ? p->obs_n_feat : (p->obs_features == 7 ? 7 : 5));
+// n_substeps == 0: one RacetrackEnv.step; n_substeps > 0: that many substeps with the persisting action, nothing else
+int launch_racetrack(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRacetrackParams& rp,
+                     const HwyNetState* s, const float* action, int n_substeps, float* obs, double* reward,
+                     uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
+                     cudaStream_t st) {
+    constexpr int G = HWY_NET_GROUP;
+    const StepPlan plan = step_plan<G, false>(s->n_envs);
+    if (configure_smem(hwynet::racetrack_step_kernel<G>, stage_smem_bytes<G, false>(hwynet::kStepThreads / G))) return 1;
+    hwynet::racetrack_step_kernel<G><<<plan.blocks, plan.threads, plan.smem, st>>>(
+        *p, graph, rp, *s, action, n_substeps, obs, reward, terminated, truncated, info_speed, info_crashed);
+    return check_launch("racetrack_step_kernel");
 }
 
-int hwy_network_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s,
-                     const int32_t* action, float* obs, double* reward, uint8_t* terminated,
-                     uint8_t* truncated, double* info_speed, uint8_t* info_crashed, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!action || !obs || !reward || !terminated || !truncated) return fail("%s", "null pointer");
-    if (s->vp != HWY_NET_GROUP) return fail("%s", "hwy_network_step expects slot stride 8 (use hwy_intersection_step)");
-    HwyIntersectionSpawn none = {};
-    return launch_step<HWY_NET_GROUP, false>(p, graph, none, s, action, obs, reward, terminated, truncated,
-                                             info_speed, info_crashed, (cudaStream_t)stream);
-}
-
-int hwy_intersection_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
-                          const HwyNetState* s, const int32_t* action, float* obs, double* reward,
-                          uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                          double* agents_reward, uint8_t* agents_terminated, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
+// The 32-slot step.  spawn == NULL (exit-v0, the 32-slot roundabout-generic): every env on 32 slots, no spawns.
+int intersection_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
+                      const HwyNetState* s, const int32_t* action, float* obs, double* reward, uint8_t* terminated,
+                      uint8_t* truncated, double* info_speed, uint8_t* info_crashed, double* agents_reward,
+                      uint8_t* agents_terminated, cudaStream_t st) {
     if (p->n_agents > 1 && (p->obs_type != HWY_OBS_KINEMATICS || p->reward_type != 1))
         return fail("%s", "several controlled vehicles: Kinematics observation on intersection envs only");
     if (!action || !obs || !reward || !terminated || !truncated) return fail("%s", "null pointer");
-    if (s->vp != HWY_NET_GROUP_LARGE) return fail("%s", "hwy_intersection_step expects slot stride 32");
     if (p->dynamic_population && (!spawn || !spawn->route_table || !spawn->route_len || !s->rng))
         return fail("%s", "dynamic population needs the spawn tables and the rng words");
     HwyIntersectionSpawn none = {};
-    cudaStream_t st = (cudaStream_t)stream;
     if (spawn && spawn->scratch && s->count) {
         // populations of <= 15 vehicles (nearly all envs) step two per warp on 16 slots, the others on 32
         int* small = spawn->scratch;
@@ -2821,26 +2828,132 @@ int hwy_intersection_step(const HwyNetParams* p, const HwyNetGraph* graph, const
                                                   agents_terminated);
 }
 
-int hwy_intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyIntersectionSpawn* spawn,
-                           const HwyNetState* s, const uint8_t* mask_a, const uint8_t* mask_b, float* obs,
-                           float* final_obs, void* stream) {
+// The scenario checks that need no device: they run before validate_net's device query
+int check_scenario(const HwyNetScenario* sc) {
+    if (sc && (sc->kind < HWY_SCENARIO_NONE || sc->kind > HWY_SCENARIO_RACETRACK))
+        return fail("%s", "unknown scenario kind");
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int hwy_network_obs_size(const HwyNetParams* p) {
+    if (!p) return 0;
+    const int agents = p->n_agents > 1 ? p->n_agents : 1;  // one observation per controlled vehicle
+    if (p->obs_type == HWY_OBS_OCCUPANCY) return agents * 4 * 11 * 11;
+    if (p->obs_type == HWY_OBS_TTC) return agents * 9 * (int)(p->ttc_horizon / (1.0 / p->policy_frequency));
+    return agents * p->obs_vehicles_count * (p->obs_n_feat > 0 ? p->obs_n_feat : (p->obs_features == 7 ? 7 : 5));
+}
+
+int hwy_network_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetScenario* sc, const HwyNetState* s,
+                      const uint8_t* mask_a, const uint8_t* mask_b, float* obs, float* final_obs, void* stream) {
+    if (!sc) return fail("%s", "null scenario: a reset needs one");
+    if (check_scenario(sc)) return 1;
+    if (sc->kind == HWY_SCENARIO_NONE) return fail("%s", "scenario kind NONE has no reset");
+    if (s && !s->rng) return fail("%s", "null rng: every reset draws from s->rng");
     if (validate_net(p, graph, s)) return 1;
-    if (s->vp != HWY_NET_GROUP_LARGE) return fail("%s", "hwy_intersection_reset expects slot stride 32");
-    if (!spawn || !spawn->route_table || !spawn->route_len || !spawn->scratch || !s->rng)
-        return fail("%s", "reset needs the spawn tables, the scratch list and the rng words");
-    if (spawn->initial_vehicle_count < 1 || spawn->initial_vehicle_count > HWY_NET_GROUP_LARGE - 2)
-        return fail("%s", "initial_vehicle_count out of range");
     if (final_obs && !obs) return fail("%s", "final_obs without obs");
     cudaStream_t st = (cudaStream_t)stream;
-    cudaMemsetAsync(spawn->scratch, 0, sizeof(int), st);
-    hwynet::compact_envs_kernel<<<(s->n_envs + 255) / 256, 256, 0, st>>>(mask_a, mask_b, s->n_envs, spawn->scratch);
-    if (final_obs)
-        cudaMemcpyAsync(final_obs, obs, (size_t)s->n_envs * hwy_network_obs_size(p) * sizeof(float),
-                        cudaMemcpyDeviceToDevice, st);
-    if (check_launch("compact_envs_kernel")) return 1;
-    if (spawn->initial_vehicle_count + 1 <= 16)  // n-1 draws + challenger + controlled vehicle fit 16 slots
-        return launch_intersection_reset<16>(p, graph, spawn, s, obs, st);
-    return launch_intersection_reset<HWY_NET_GROUP_LARGE>(p, graph, spawn, s, obs, st);
+    switch (sc->kind) {
+    case HWY_SCENARIO_ROUNDABOUT: {
+        const HwyRoundaboutSpawn& sp = sc->u.roundabout;
+        if (!sp.route_table || !sp.route_len) return fail("%s", "null route table");
+        if (p->n_vehicles != 5 || s->vp != HWY_NET_GROUP) return fail("%s", "roundabout spawn places exactly 5 vehicles in 8 slots");
+        return scripted_reset(hwynet::roundabout_reset_kernel, "roundabout_reset_kernel", 32,  // a warp per env
+                              p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
+    case HWY_SCENARIO_ROUNDABOUT_GENERIC: {
+        const HwyRoundaboutGenericSpawn& sp = sc->u.roundabout_generic;
+        if (!sp.route_table || !sp.route_len) return fail("%s", "null route table");
+        if (!s->count) return fail("%s", "roundabout-generic: the count buffer receives the population");
+        if (sp.vehicles_count > s->vp - 1 || p->n_vehicles < 1 + (sp.vehicles_count > 0 ? sp.vehicles_count : 0))
+            return fail("%s", "roundabout-generic: vehicles_count exceeds the slots or n_vehicles");
+        if (sp.fixed_destination < -1 || sp.fixed_destination > 3 || sp.route_width < 5)
+            return fail("%s", "roundabout-generic: fixed_destination out of -1..3 or route_width < 5");
+        if (sp.ego_lane < 0 || sp.ego_lane >= HWY_NET_MAX_LANES) return fail("%s", "ego_lane out of range");
+        for (int k = 0; k < 7; ++k)
+            if (sp.spawn_road[k] < 0 || sp.spawn_road[k] >= HWY_NET_MAX_LANES) return fail("%s", "spawn_road out of range");
+        return scripted_reset(hwynet::roundabout_generic_reset_kernel, "roundabout_generic_reset_kernel", 32,
+                              p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
+    case HWY_SCENARIO_MERGE:
+        if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "merge-v0: 5 vehicles + 1 obstacle on 8 slots");
+        return scripted_reset(hwynet::merge_reset_kernel, "merge_reset_kernel", 1,
+                              p, graph, sc->u.merge, s, mask_a, mask_b, obs, final_obs, st);
+    case HWY_SCENARIO_TWO_WAY:
+        if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "two-way-v0: 6 vehicles on 8 slots");
+        return scripted_reset(hwynet::two_way_reset_kernel, "two_way_reset_kernel", 1,
+                              p, graph, sc->u.two_way, s, mask_a, mask_b, obs, final_obs, st);
+    case HWY_SCENARIO_U_TURN: {
+        const HwyUTurnSpawn& sp = sc->u.u_turn;
+        if (!sp.route_table || !sp.route_len) return fail("%s", "null route table");
+        if (s->vp != HWY_NET_GROUP || p->n_vehicles != 7) return fail("%s", "u-turn-v0: 7 vehicles on 8 slots");
+        return scripted_reset(hwynet::u_turn_reset_kernel, "u_turn_reset_kernel", 1,
+                              p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
+    case HWY_SCENARIO_EXIT: {
+        const HwyExitSpawn& sp = sc->u.exit;
+        if (s->vp != HWY_NET_GROUP_LARGE || sp.n_vehicles < 1 || sp.n_vehicles > HWY_NET_GROUP_LARGE)
+            return fail("%s", "exit-v0: 1..32 vehicles on 32 slots");
+        if (sp.lanes_count < 1 || sp.lanes_count > HWY_MAX_LANES) return fail("%s", "lanes_count out of range");
+        return scripted_reset(hwynet::exit_reset_kernel, "exit_reset_kernel", 1,
+                              p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
+    case HWY_SCENARIO_INTERSECTION: {
+        const HwyIntersectionSpawn& sp = sc->u.intersection;
+        if (s->vp != HWY_NET_GROUP_LARGE) return fail("%s", "the intersection reset expects slot stride 32");
+        if (!sp.route_table || !sp.route_len || !sp.scratch)
+            return fail("%s", "the intersection reset needs the spawn tables and the scratch list");
+        if (sp.initial_vehicle_count < 1 || sp.initial_vehicle_count > HWY_NET_GROUP_LARGE - 2)
+            return fail("%s", "initial_vehicle_count out of range");
+        return intersection_reset(p, graph, &sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
+    default:  // HWY_SCENARIO_RACETRACK
+        if (validate_racetrack(p, &sc->u.racetrack, s)) return 1;
+        return scripted_reset(hwynet::racetrack_reset_kernel, "racetrack_reset_kernel", 1,
+                              p, graph, sc->u.racetrack, s, mask_a, mask_b, obs, final_obs, st);
+    }
+}
+
+int hwy_network_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetScenario* sc, const HwyNetState* s,
+                     const void* action, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
+                     double* info_speed, uint8_t* info_crashed, double* agents_reward, uint8_t* agents_terminated,
+                     void* stream) {
+    if (check_scenario(sc) || validate_net(p, graph, s)) return 1;
+    const int kind = sc ? sc->kind : HWY_SCENARIO_NONE;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (kind == HWY_SCENARIO_RACETRACK) {
+        if (validate_racetrack(p, &sc->u.racetrack, s)) return 1;
+        if (!action || !obs || !reward || !terminated || !truncated) return fail("%s", "null pointer");
+        return launch_racetrack(p, graph, sc->u.racetrack, s, (const float*)action, 0, obs, reward, terminated,
+                                truncated, info_speed, info_crashed, st);
+    }
+    if (s->vp == HWY_NET_GROUP_LARGE)
+        return intersection_step(p, graph, kind == HWY_SCENARIO_INTERSECTION ? &sc->u.intersection : nullptr, s,
+                                 (const int32_t*)action, obs, reward, terminated, truncated, info_speed, info_crashed,
+                                 agents_reward, agents_terminated, st);
+    if (!action || !obs || !reward || !terminated || !truncated) return fail("%s", "null pointer");
+    HwyIntersectionSpawn none = {};
+    return launch_step<HWY_NET_GROUP, false>(p, graph, none, s, (const int32_t*)action, obs, reward, terminated,
+                                             truncated, info_speed, info_crashed, st);
+}
+
+int hwy_network_substeps(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetScenario* sc,
+                         const HwyNetState* s, const uint8_t* mask, int n_substeps, void* stream) {
+    if (check_scenario(sc)) return 1;
+    const bool racetrack = sc && sc->kind == HWY_SCENARIO_RACETRACK;
+    if (racetrack && mask) return fail("%s", "racetrack substeps run every env: mask must be NULL");
+    if (validate_net(p, graph, s) || (racetrack && validate_racetrack(p, &sc->u.racetrack, s))) return 1;
+    if (n_substeps < 0) return fail("%s", "n_substeps < 0");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (racetrack)  // the racetrack kernel reads n_substeps == 0 as a policy step: nothing to launch
+        return n_substeps ? launch_racetrack(p, graph, sc->u.racetrack, s, nullptr, n_substeps, nullptr, nullptr,
+                                             nullptr, nullptr, nullptr, nullptr, st)
+                          : 0;
+    return launch_groups([](auto t) { return hwynet::network_substeps_kernel<decltype(t)::G, decltype(t)::REG>; },
+                         "network_substeps_kernel", s, st, *p, graph, *s, mask, n_substeps);
 }
 
 int hwy_debug_network_neighbours(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s,
@@ -2866,109 +2979,11 @@ int hwy_debug_rotated_rectangles_intersect(const double* rects, int n, int32_t* 
     return check_launch("debug_rectangles_kernel");
 }
 
-int hwy_merge_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyMergeSpawn* spawn, const HwyNetState* s,
-                    uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng) return fail("%s", "null spawn / rng");
-    if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "merge-v0: 5 vehicles + 1 obstacle on 8 slots");
-    return scripted_reset(hwynet::merge_reset_kernel, "merge_reset_kernel", 1,
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_exit_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyExitSpawn* spawn, const HwyNetState* s,
-                   uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng) return fail("%s", "null spawn / rng");
-    if (s->vp != HWY_NET_GROUP_LARGE || spawn->n_vehicles < 1 || spawn->n_vehicles > HWY_NET_GROUP_LARGE)
-        return fail("%s", "exit-v0: 1..32 vehicles on 32 slots");
-    if (spawn->lanes_count < 1 || spawn->lanes_count > HWY_MAX_LANES) return fail("%s", "lanes_count out of range");
-    return scripted_reset(hwynet::exit_reset_kernel, "exit_reset_kernel", 1,
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_u_turn_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyUTurnSpawn* spawn, const HwyNetState* s,
-                     uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng / route table");
-    if (s->vp != HWY_NET_GROUP || p->n_vehicles != 7) return fail("%s", "u-turn-v0: 7 vehicles on 8 slots");
-    return scripted_reset(hwynet::u_turn_reset_kernel, "u_turn_reset_kernel", 1,
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_two_way_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyTwoWaySpawn* spawn, const HwyNetState* s,
-                      uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng) return fail("%s", "null spawn / rng");
-    if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "two-way-v0: 6 vehicles on 8 slots");
-    return scripted_reset(hwynet::two_way_reset_kernel, "two_way_reset_kernel", 1,
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_racetrack_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRacetrackParams* rp,
-                        const HwyNetState* s, uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b, float* obs,
-                        void* stream) {
-    if (validate_net(p, graph, s) || validate_racetrack(p, rp, s)) return 1;
-    if (!rng) return fail("%s", "null rng");
-    return scripted_reset(hwynet::racetrack_reset_kernel, "racetrack_reset_kernel", 1,
-                          p, graph, rp, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_racetrack_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRacetrackParams* rp,
-                       const HwyNetState* s, const float* action, int n_substeps, float* obs, double* reward,
-                       uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                       void* stream) {
-    if (validate_net(p, graph, s) || validate_racetrack(p, rp, s)) return 1;
-    if (n_substeps < 0) return fail("%s", "n_substeps < 0");
-    if (n_substeps == 0 && (!action || !obs || !reward || !terminated || !truncated)) return fail("%s", "null pointer");
-    constexpr int G = HWY_NET_GROUP;
-    const StepPlan plan = step_plan<G, false>(s->n_envs);
-    if (configure_smem(hwynet::racetrack_step_kernel<G>, stage_smem_bytes<G, false>(hwynet::kStepThreads / G))) return 1;
-    hwynet::racetrack_step_kernel<G><<<plan.blocks, plan.threads, plan.smem, (cudaStream_t)stream>>>(
-        *p, graph, *rp, *s, action, n_substeps, obs, reward, terminated, truncated, info_speed, info_crashed);
-    return check_launch("racetrack_step_kernel");
-}
-
-int hwy_network_substeps(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, const uint8_t* mask,
-                         int n_substeps, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (n_substeps < 0) return fail("%s", "n_substeps < 0");
-    return launch_groups([](auto t) { return hwynet::network_substeps_kernel<decltype(t)::G, decltype(t)::REG>; },
-                         "network_substeps_kernel", s, (cudaStream_t)stream, *p, graph, *s, mask, n_substeps);
-}
-
 int hwy_network_observe(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetState* s, float* obs,
                         void* stream) {
     if (validate_net(p, graph, s)) return 1;
     if (!obs) return fail("%s", "obs is null");
     return observe_dispatch(p, graph, s, nullptr, nullptr, obs, (cudaStream_t)stream);
-}
-
-int hwy_roundabout_reset(const HwyNetParams* p, const HwyNetGraph* graph, const HwyRoundaboutSpawn* spawn,
-                         const HwyNetState* s, uint64_t* rng, const uint8_t* mask_a, const uint8_t* mask_b,
-                         float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng pointer");
-    if (p->n_vehicles != 5 || s->vp != HWY_NET_GROUP) return fail("%s", "roundabout spawn places exactly 5 vehicles in 8 slots");
-    return scripted_reset(hwynet::roundabout_reset_kernel, "roundabout_reset_kernel", 32,  // a warp per env
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
-}
-
-int hwy_roundabout_generic_reset(const HwyNetParams* p, const HwyNetGraph* graph,
-                                 const HwyRoundaboutGenericSpawn* spawn, const HwyNetState* s, uint64_t* rng,
-                                 const uint8_t* mask_a, const uint8_t* mask_b, float* obs, void* stream) {
-    if (validate_net(p, graph, s)) return 1;
-    if (!spawn || !rng || !spawn->route_table || !spawn->route_len) return fail("%s", "null spawn / rng pointer");
-    if (!s->count) return fail("%s", "roundabout-generic: the count buffer receives the population");
-    if (spawn->vehicles_count > s->vp - 1 || p->n_vehicles < 1 + (spawn->vehicles_count > 0 ? spawn->vehicles_count : 0))
-        return fail("%s", "roundabout-generic: vehicles_count exceeds the slots or n_vehicles");
-    if (spawn->fixed_destination < -1 || spawn->fixed_destination > 3 || spawn->route_width < 5)
-        return fail("%s", "roundabout-generic: fixed_destination out of -1..3 or route_width < 5");
-    if (spawn->ego_lane < 0 || spawn->ego_lane >= HWY_NET_MAX_LANES) return fail("%s", "ego_lane out of range");
-    for (int k = 0; k < 7; ++k)
-        if (spawn->spawn_road[k] < 0 || spawn->spawn_road[k] >= HWY_NET_MAX_LANES)
-            return fail("%s", "spawn_road out of range");
-    return scripted_reset(hwynet::roundabout_generic_reset_kernel, "roundabout_generic_reset_kernel", 32,
-                          p, graph, spawn, s, rng, mask_a, mask_b, obs, stream);
 }
 
 }  // extern "C"

@@ -5,8 +5,9 @@
 ``seed + env_index_offset + i`` would own), ``reset`` / ``step`` with the three autoreset modes, action staging,
 standalone observation plugins and ``state_dict``.  A family supplies its kernels through ``_step_kernels``,
 ``_device_reset`` and ``_observe_kernel``.  ``BatchedNetworkEnv`` adds what the general-network families
-(roundabout, merge, two-way, u-turn, exit, intersection) share: the lane table on the device, the ``HwyNetState``
-buffers, ``road_substeps`` and the numpy-exact host reset mode.
+(roundabout, merge, two-way, u-turn, exit, intersection, racetrack) share: the lane table on the device, the
+``HwyNetState`` buffers, the kernels of the family's ``HwyNetScenario``, ``road_substeps`` and the numpy-exact host
+reset mode.
 
 The env streams always live on the device as 5 words per env (state hi, lo, inc hi, lo, has_uint32 << 32 |
 uinteger); a host reset borrows numpy generators for the envs it re-spawns and writes their words back.
@@ -401,8 +402,9 @@ class BatchedVectorEnv:
 
 
 class BatchedNetworkEnv(BatchedVectorEnv):
-    """The general-network families: a lane table on the device (``_make_network``), the ``HwyNetState`` buffers,
-    ``hwy_network_observe`` / ``hwy_network_substeps`` and two reset modes.
+    """The general-network families: a lane table on the device (``_make_network``), the ``HwyNetState`` buffers, and
+    the network reset / step / substeps entry points, which read the family's ``HwyNetScenario`` (``_scenario``, built
+    with its spawn constants), and two reset modes.
 
     * ``reset_mode="device"`` (default): the family's reset kernel re-spawns from the env streams; SameStep autoreset
       stays on the device.
@@ -412,6 +414,7 @@ class BatchedNetworkEnv(BatchedVectorEnv):
     SLOTS = N.HWY_NET_GROUP  # vehicle slots per env: 8 (one warp serves four envs) or 32 (HWY_NET_GROUP_LARGE)
     n_agents = 1
     multi_agent = False
+    _pair_buf = None  # racetrack with one control axis: the (throttle, steering) pairs the step reads instead of act
 
     def __init__(self, config: Optional[dict] = None, render_mode: Optional[str] = None, num_envs: int = 1,
                  device: Any = None, autoreset_mode: str = "SameStep", env_index_offset: int = 0,
@@ -463,7 +466,7 @@ class BatchedNetworkEnv(BatchedVectorEnv):
         st.delta, st.meta = self._delta.data_ptr(), self._meta.data_ptr()
         st.route, st.route_len = self._route.data_ptr(), self._route_len.data_ptr()
         st.speed_index, st.time = self._speed_index.data_ptr(), self._time.data_ptr()
-        st.reward_terms = self._reward_terms.data_ptr()
+        st.reward_terms, st.rng = self._reward_terms.data_ptr(), self._rng.data_ptr()
         self._state = st
         return st
 
@@ -518,9 +521,30 @@ class BatchedNetworkEnv(BatchedVectorEnv):
         idx = torch.from_numpy(np.asarray(ids, dtype=np.int64)).to(self.device)
         self._rng[:, idx] = torch.from_numpy(pcg64_words(generators).view(np.int64)).to(self.device)
 
+    def _device_reset(self, mask_a, mask_b, obs_ptr, final_obs_ptr=None) -> None:
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_network_reset(
+                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._scenario), C.byref(self._state),
+                mask_a, mask_b, obs_ptr, final_obs_ptr, self._stream()))
+
+    def _step_kernels(self, act) -> None:
+        act = act if self._pair_buf is None else self._pair_buf
+        agents = self.multi_agent
+        with torch.cuda.device(self.device):
+            N.check(self._lib.hwy_network_step(
+                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._scenario), C.byref(self._state),
+                act.data_ptr(), self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
+                self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
+                self._agents_reward.data_ptr() if agents else None,
+                self._agents_terminated.data_ptr() if agents else None, self._stream()))
+
     def _same_step_autoreset(self, info) -> None:
         if self.reset_mode == "device":
-            return super()._same_step_autoreset(info)
+            if self._plugin_standalone:
+                return super()._same_step_autoreset(info)
+            info["final_obs"] = self._out_final_obs()  # the reset copies the fused observation there first
+            return self._device_reset(self._terminated.data_ptr(), self._truncated.data_ptr(), self._obs.data_ptr(),
+                                      self._final_obs.data_ptr())
         done = (self._terminated | self._truncated).cpu().numpy().astype(bool)
         if done.any():
             self._final_obs.copy_(self._obs)
@@ -532,9 +556,13 @@ class BatchedNetworkEnv(BatchedVectorEnv):
         """The reference's operator seam (`AbstractEnv._simulate` without `action_type.act`, abstract.py:304-307):
         `n_substeps` x (`Road.act()`; `Road.step(1 / simulation_frequency)`, with the RegulatedRoad rules where the
         scenario has them) on the device state of every env and nothing else — no observation, reward, clock,
-        population change or autoreset; the controlled vehicle acts like `ControlledVehicle.act(None)`."""
+        population change or autoreset; the controlled vehicle acts like `ControlledVehicle.act(None)`, or a plain
+        Vehicle ego keeps the action of its last step (Vehicle.act(None), kinematics.py:119-128)."""
         if not self._seeded:
             raise RuntimeError("call reset() before road_substeps()")
+        if n_substeps < 0 and self._scenario.kind == N.HWY_SCENARIO_RACETRACK:
+            raise ValueError("n_substeps < 0")
         with torch.cuda.device(self.device):
             N.check(self._lib.hwy_network_substeps(C.byref(self._params), self._graph_dev.data_ptr(),
-                                                   C.byref(self._state), None, int(n_substeps), self._stream()))
+                                                   C.byref(self._scenario), C.byref(self._state), None,
+                                                   int(n_substeps), self._stream()))

@@ -7,7 +7,7 @@ Host-side mirror of the reference's ``ExitEnv`` (highway_env/envs/exit_env.py:15
 envs/common/observation.py:624-675); reward with a goal term for targeting the exit lane (:147-198).
 
 21 vehicles need the 32-slot network kernels (the intersection family's `network_step_kernel<32>` without rules or
-population changes); reset is ``hwy_exit_reset`` on the env's numpy stream (weighted `choice(p=...)` + `uniform`).
+population changes); the device reset draws from the env's numpy stream (weighted `choice(p=...)` + `uniform`).
 """
 from __future__ import annotations
 
@@ -52,7 +52,6 @@ def make_exit_network(lanes_count: int = 6, road_length: float = 1000, exit_posi
 
 class BatchedExitEnv(BatchedRoundaboutEnv):
     ENV_ID = "exit-v0"
-    RESET_ENTRY = "hwy_exit_reset"
     SLOTS = N.HWY_NET_GROUP_LARGE
     N_VEHICLES = 21
     REWARD_NAMES = ("collision_reward", "goal_reward", "high_speed_reward", "right_lane_reward")  # _rewards :164-176
@@ -77,7 +76,7 @@ class BatchedExitEnv(BatchedRoundaboutEnv):
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError("exit envs reset on the device (hwy_exit_reset)")
+            raise NotImplementedError("exit envs reset on the device")
         cfg = self.config
         if cfg.get("other_vehicles_type") != "highway_env.vehicle.behavior.IDMVehicle":
             raise NotImplementedError("only IDMVehicle traffic is on the accelerated path")
@@ -110,7 +109,7 @@ class BatchedExitEnv(BatchedRoundaboutEnv):
             s.cdf[k] = float(cdf[k])
         s.route_12 = int(net.encode_route([("1", "2", None)])[0][0])
         s.route_23 = int(net.encode_route([("2", "3", None)])[0][0])
-        self._spawn_struct = s
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_EXIT, u=N.HwyNetScenarioUnion(exit=s))
 
     def _step_result(self, info):
         info["is_success"] = self._reward_terms[:, 1] > 0  # ExitEnv.step (:51-54): info["is_success"]

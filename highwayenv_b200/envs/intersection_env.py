@@ -6,10 +6,10 @@ changes every step (``_clear_vehicles`` / ``_spawn_vehicle``), Kinematics (7 fea
 OccupancyGrid observation, 3 longitudinal meta-actions.
 
 Stepping — including the RegulatedRoad rules and the per-step clear/spawn with the env's numpy
-stream — runs in ``hwy_intersection_step``.  ``reset`` has two implementations of
+stream — runs in ``hwy_network_step`` (HWY_SCENARIO_INTERSECTION).  ``reset`` has two implementations of
 ``_make_vehicles`` (:245-323):
 
-* ``reset_mode="device"`` (default): ``hwy_intersection_reset`` — draws, warm-up simulation,
+* ``reset_mode="device"`` (default): ``hwy_network_reset`` — draws, warm-up simulation,
   challenger, controlled vehicle and pruning in one kernel over the envs that finished; this is
   what the SameStep autoreset uses, so a step never leaves the GPU.
 * ``reset_mode="host"``: the same sequence with numpy generators on the host (bit-identical to
@@ -82,6 +82,11 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
 
     def _make_network(self) -> NetworkTable:
         return make_intersection_network()
+
+    @property
+    def _spawn_struct(self) -> N.HwyIntersectionSpawn:
+        """The scenario's spawn constants and work lists, a view into `_scenario`: writes reach the kernels."""
+        return self._scenario.u.intersection
 
     # ------------------------------------------------------------------ spaces / parameters
     def define_spaces(self) -> None:
@@ -181,7 +186,7 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
             self._action_buf = z(n, 2, dtype=torch.float32)
         else:
             self._action_buf = z(n, A, dtype=torch.int32) if self.multi_agent else z(n, dtype=torch.int32)
-        st.count, st.road_steps, st.rng = self._count.data_ptr(), self._road_steps.data_ptr(), self._rng.data_ptr()
+        st.count, st.road_steps = self._count.data_ptr(), self._road_steps.data_ptr()
         st.overflow = self._overflow.data_ptr()
         self._routes, self._route_lens = self._route_tables(["o0", "o1", "o2", "o3"])
         sp = N.HwyIntersectionSpawn()
@@ -197,7 +202,7 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
         sp.initial_vehicle_count = int(self.config["initial_vehicle_count"])
         self._scratch = z(2 * (n + 1), dtype=torch.int32)
         sp.scratch = self._scratch.data_ptr()
-        self._spawn_struct = sp
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_INTERSECTION, u=N.HwyNetScenarioUnion(intersection=sp))
 
     # ------------------------------------------------------------------ state import / export
     def state_dict(self) -> dict:
@@ -288,7 +293,7 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
         mask[torch.from_numpy(np.asarray(ids, dtype=np.int64)).to(self.device)] = 1
         with torch.cuda.device(self.device):
             N.check(self._lib.hwy_network_substeps(C.byref(self._params), self._graph_dev.data_ptr(),
-                                                   C.byref(self._state), mask.data_ptr(),
+                                                   C.byref(self._scenario), C.byref(self._state), mask.data_ptr(),
                                                    3 * int(cfg["simulation_frequency"]), self._stream()))
         full = self.state_dict()
         sd = {k: (v[ids].copy() if k != "rng" else None) for k, v in full.items()}
@@ -319,24 +324,8 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
             sd["time"][k] = 0.0
         self.load_state_dict(sd, ids)
 
-    # ------------------------------------------------------------------ family kernels
-    def _device_reset(self, mask_a, mask_b, obs_ptr, final_obs_ptr=None) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_intersection_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                mask_a, mask_b, obs_ptr, final_obs_ptr, self._stream()))
-
     def _reset_info(self) -> dict:
         return {"speed": self._info_speed, "crashed": self._info_crashed.view(torch.bool)}
-
-    def _step_kernels(self, act) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_intersection_step(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct), C.byref(self._state),
-                act.data_ptr(), self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
-                self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
-                self._agents_reward.data_ptr() if self.multi_agent else None,
-                self._agents_terminated.data_ptr() if self.multi_agent else None, self._stream()))
 
     def _step_info(self, act) -> dict:
         info = super()._step_info(act)
@@ -348,13 +337,6 @@ class BatchedIntersectionEnv(BatchedNetworkEnv):
             info["agents_rewards"] = self._agents_reward
             info["agents_terminated"] = self._agents_terminated.view(torch.bool)
         return info
-
-    def _same_step_autoreset(self, info) -> None:
-        if self.reset_mode != "device" or self._plugin_standalone:
-            return super()._same_step_autoreset(info)
-        info["final_obs"] = self._final_obs  # the reset kernel writes the final observation of the finished envs
-        self._device_reset(self._terminated.data_ptr(), self._truncated.data_ptr(), self._obs.data_ptr(),
-                           self._final_obs.data_ptr())
 
     def _step_result(self, info):
         if self.multi_agent and self.MULTI_AGENT_WRAPPER:

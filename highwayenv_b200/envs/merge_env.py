@@ -49,7 +49,6 @@ def make_merge_network() -> NetworkTable:
 
 class BatchedMergeEnv(BatchedRoundaboutEnv):
     ENV_ID = "merge-v0"
-    RESET_ENTRY = "hwy_merge_reset"
     N_VEHICLES = 6  # five vehicles + the Obstacle
     EGO_SIDE_LANES = 2  # the controlled vehicle spawns on ("a", "b", 1): normalize_obs' default y-range (observation.py:214-226)
     REWARD_NAMES = ("collision_reward", "right_lane_reward", "high_speed_reward", "lane_change_reward", "merging_speed_reward")  # _rewards :62-77
@@ -59,7 +58,7 @@ class BatchedMergeEnv(BatchedRoundaboutEnv):
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError("merge envs reset on the device (hwy_merge_reset)")
+            raise NotImplementedError("merge envs reset on the device")
         cfg = self.config
         cfg.setdefault("normalize_reward", False)
         cfg.setdefault("duration", float("inf"))  # AbstractEnv has no duration; MergeEnv never truncates
@@ -81,7 +80,7 @@ class BatchedMergeEnv(BatchedRoundaboutEnv):
         s.ego_speed_index = speed_to_index(ts, 30.0)
         ox, oy = net.position(net.index[("b", "c", 2)], 80.0, 0.0)
         s.obstacle_x, s.obstacle_y = float(ox), float(oy)
-        self._spawn_struct = s
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_MERGE, u=N.HwyNetScenarioUnion(merge=s))
 
 
 class BatchedConnectedLaneMergeEnv(BatchedMergeEnv):

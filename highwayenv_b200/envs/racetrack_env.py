@@ -7,18 +7,17 @@ track of 9 roads (straight and circular, width 5, speed limit 10), one controlle
 default observation is a 12 x 12 OccupancyGrid (presence, on_road) aligned with the vehicle, observed by the standalone
 grid kernel; Kinematics is written by the step kernel itself.
 
-Stepping runs in ``hwy_racetrack_step`` (include/hwyb200.h) on the 8-slot network state: the network kernels' substep
-with a plain ego, then the racetrack reward (:66-83), termination (crash, or off road with ``terminate_off_road``) and
-truncation at ``duration``.  Resets run in ``hwy_racetrack_reset`` from each env's numpy stream, in the reference's
-draw order (:374-425).  The plain Vehicle's action dict persists between steps (kinematics.py:119-128): the state
-keeps it in the ego's (target_speed, timer) pair as (acceleration, steering), which ``road_substeps`` replays.
+Stepping runs in ``hwy_network_step`` with HWY_SCENARIO_RACETRACK (include/hwyb200.h) on the 8-slot network state:
+the network kernels' substep with a plain ego, then the racetrack reward (:66-83), termination (crash, or off road with
+``terminate_off_road``) and truncation at ``duration``.  Resets run in ``hwy_network_reset`` from each env's numpy
+stream, in the reference's draw order (:374-425).  The plain Vehicle's action dict persists between steps
+(kinematics.py:119-128): the state keeps it in the ego's (target_speed, timer) pair as (acceleration, steering), which
+``road_substeps`` replays.
 
 The large track (``RacetrackEnvLarge``, 9 roads x 3 lanes) and the oval (``RacetrackEnvOval``, 8 roads x ``no_lanes``)
 run on the same kernels with their own lane tables; only the ego's lane draw differs (``HwyRacetrackParams.ego_lanes``).
 """
 from __future__ import annotations
-
-import ctypes as C
 
 import numpy as np
 import torch
@@ -277,7 +276,7 @@ def racetrack_params(cfg: dict, env_id: str = "racetrack-v0") -> dict:
     # the ego's lane draw: integers(2) in RacetrackEnv._make_vehicles (also the large track's), integers(no_lanes) in
     # the oval's; the front vehicle takes the same lane id on ("b","c")
     rp.ego_lanes = int(cfg["no_lanes"]) if oval else 2
-    # hwy_racetrack_reset cannot read the device table; the lane ids it draws must exist on both roads
+    # the reset cannot read the device table; the lane ids it draws must exist on both roads
     if rp.ego_lanes > min(net.lanes[rp.lane_ab]["road_count"], net.lanes[rp.lane_bc]["road_count"]):
         raise ValueError(f"ego_lanes {rp.ego_lanes} exceeds the lanes of ('a','b') or ('b','c') on {env_id}")
     rp.lane_centering_cost = float(cfg["lane_centering_cost"])
@@ -299,17 +298,24 @@ class BatchedRacetrackEnv(BatchedNetworkEnv):
     def _make_network(self) -> NetworkTable:
         return self._track
 
+    @property
+    def _race(self) -> N.HwyRacetrackParams:
+        """The scenario's racetrack parameters, a view into `_scenario`: writes reach the kernels."""
+        return self._scenario.u.racetrack
+
     # ------------------------------------------------------------------ configuration
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError(f"{self.ENV_ID} resets on the device (hwy_racetrack_reset)")
+            raise NotImplementedError(f"{self.ENV_ID} resets on the device")
         spec = racetrack_params(self.config, self.ENV_ID)
         # the lane table follows the config (the oval's length / no_lanes, the large track's speed_limit): after
         # reset(options={"config": ...}) picks another track, `net` rebuilds the table and its device copy
         if self._net is not spec["net"]:
             self._net = None
         self._track = spec["net"]
-        self._params, self._race = spec["params"], spec["race"]
+        self._params = spec["params"]
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_RACETRACK,
+                                          u=N.HwyNetScenarioUnion(racetrack=spec["race"]))
         self.action_type, self.observation_type = spec["action_type"], spec["observation_type"]
         self.lateral, self.action_size, self.V = spec["lateral"], spec["action_size"], spec["V"]
         self._plugin_standalone = not spec["fused"]
@@ -335,36 +341,6 @@ class BatchedRacetrackEnv(BatchedNetworkEnv):
         if self._pair_buf is not None:  # one control axis: the other stays 0
             self._pair_buf[:, 1 if self.lateral else 0].copy_(act[:, 0])
         return act
-
-    # ------------------------------------------------------------------ family kernels
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_racetrack_reset(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
-                self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
-
-    def _step_kernels(self, act) -> None:
-        pairs = act if self._pair_buf is None else self._pair_buf
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_racetrack_step(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
-                pairs.data_ptr(), 0, self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
-                self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
-                self._stream()))
-
-    def road_substeps(self, n_substeps: int) -> None:
-        """`n_substeps` x (Road.act(); Road.step(1 / simulation_frequency)) of every env and nothing else; the plain
-        ego keeps the action of its last step (Vehicle.act(None), kinematics.py:119-128)."""
-        if not self._seeded:
-            raise RuntimeError("call reset() before road_substeps()")
-        if n_substeps < 0:
-            raise ValueError("n_substeps < 0")
-        if n_substeps == 0:
-            return
-        with torch.cuda.device(self.device):
-            N.check(self._lib.hwy_racetrack_step(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._race), C.byref(self._state),
-                None, int(n_substeps), None, None, None, None, None, None, self._stream()))
 
     def to_finite_mdp(self):
         raise NotImplementedError(f"to_finite_mdp on {self.ENV_ID}: the finite MDP needs DiscreteMetaAction")

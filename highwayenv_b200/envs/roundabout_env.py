@@ -8,7 +8,7 @@ Every env owns the numpy ``Generator(PCG64)`` stream a reference env seeded with
 ``seed + env_index_offset + i`` would own; ``_make_vehicles`` draws from it in the reference's
 order (normal, normal, choice, uniform per traffic vehicle).  Two reset modes:
 
-* ``reset_mode="device"`` (default): ``hwy_roundabout_reset`` re-spawns on the GPU from the stream
+* ``reset_mode="device"`` (default): ``hwy_network_reset`` re-spawns on the GPU from the stream
   (PCG64 + numpy's ziggurat normal restated on the device).  Draws, lanes and routes are identical
   to the reference; spawn coordinates go through CUDA's sin/cos instead of numpy's and may differ
   in the last ulp (~1e-15 m).  SameStep autoreset stays on the device.
@@ -16,11 +16,9 @@ order (normal, normal, choice, uniform per traffic vehicle).  Two reset modes:
   uploaded; autoreset round-trips through the host.
 
 roundabout-generic-v0 / v1 (``RoundaboutGenericEnv``, :398-757) run the same task on a lane table built from the
-config and reset on the device only (``hwy_roundabout_generic_reset``); see ``BatchedRoundaboutGenericEnv``.
+config and reset on the device only; see ``BatchedRoundaboutGenericEnv``.
 """
 from __future__ import annotations
-
-import ctypes as C
 
 import numpy as np
 import torch
@@ -234,7 +232,6 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
     EGO_SIDE_LANES = 1  # lanes of the road the controlled vehicle spawns on (default Kinematics y-range)
     REWARD_NAMES = ("collision_reward", "high_speed_reward", "lane_change_reward", "on_road_reward")  # _rewards :58-65
     META_FLAGS = ("crashed", "no_lane_change", "has_impact", "check_collisions")
-    RESET_ENTRY = "hwy_roundabout_reset"  # the scenario's reset kernel (same arguments for every roundabout-family env)
 
     def _make_network(self) -> NetworkTable:
         return make_roundabout_network()
@@ -308,29 +305,7 @@ class BatchedRoundaboutEnv(BatchedNetworkEnv):
         s.position_deviation, s.speed_deviation, s.traffic_speed = 2.0, 2.0, 16.0
         s.delta_lo, s.delta_hi = 3.5, 4.5
         s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
-        self._spawn_struct = s
-
-    # ------------------------------------------------------------------ family kernels
-    def _device_reset(self, mask_a, mask_b, obs_ptr) -> None:
-        with torch.cuda.device(self.device):
-            N.check(getattr(self._lib, self.RESET_ENTRY)(
-                C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._spawn_struct),
-                C.byref(self._state), self._rng.data_ptr(), mask_a, mask_b, obs_ptr, self._stream()))
-
-    def _step_kernels(self, act) -> None:
-        with torch.cuda.device(self.device):
-            if self.SLOTS == N.HWY_NET_GROUP:
-                N.check(self._lib.hwy_network_step(
-                    C.byref(self._params), self._graph_dev.data_ptr(), C.byref(self._state), act.data_ptr(),
-                    self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
-                    self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
-                    self._stream()))
-            else:  # 32 slots: the intersection family's kernel without rules / population changes
-                N.check(self._lib.hwy_intersection_step(
-                    C.byref(self._params), self._graph_dev.data_ptr(), None, C.byref(self._state), act.data_ptr(),
-                    self._fused_out.data_ptr(), self._reward.data_ptr(), self._terminated.data_ptr(),
-                    self._truncated.data_ptr(), self._info_speed.data_ptr(), self._info_crashed.data_ptr(),
-                    None, None, self._stream()))
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_ROUNDABOUT, u=N.HwyNetScenarioUnion(roundabout=s))
 
     def get_available_actions(self) -> torch.Tensor:
         """DiscreteMetaAction.get_available_actions (envs/common/action.py:262-298, AbstractEnv.get_available_actions
@@ -409,20 +384,19 @@ def check_roundabout_generic(cfg: dict, env_id: str) -> None:
 class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
     """`roundabout-generic-v0`: RoundaboutGenericEnv (roundabout_env.py:398-751), RoundaboutEnv's rewards, termination
     and dynamics on a roundabout of config["roundabout_lanes"] ring lanes (1..2) at config["roundabout_radius"], with
-    config["vehicles_count"] traffic vehicles placed by rejection sampling (``hwy_roundabout_generic_reset``).  A
+    config["vehicles_count"] traffic vehicles placed by rejection sampling (HWY_SCENARIO_ROUNDABOUT_GENERIC).  A
     vehicle whose 10 tries fail is skipped, so the population varies per env (``count``).  Up to 7 traffic vehicles
-    run on 8 slots (``hwy_network_step``), 8 to 31 on 32 slots (``hwy_intersection_step`` without rules or spawns).
+    run on 8 slots, 8 to 31 on 32 slots (the intersection family's step without rules or spawns).
     The lane table follows the config: reset(options={"config": ...}) rebuilds it and re-allocates."""
 
     ENV_ID = "roundabout-generic-v0"
-    RESET_ENTRY = "hwy_roundabout_generic_reset"
 
     def _make_network(self) -> NetworkTable:
         return self._road
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError(f"{self.ENV_ID} resets on the device ({self.RESET_ENTRY})")
+            raise NotImplementedError(f"{self.ENV_ID} resets on the device")
         cfg = self.config
         check_roundabout_generic(cfg, self.ENV_ID)
         road = roundabout_generic_network(cfg["roundabout_radius"], cfg["roundabout_lanes"])
@@ -454,7 +428,8 @@ class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
         s.ego_speed_index = speed_to_index(self.action_type.target_speeds, 8.0)
         s.route_width = table.shape[1]
         s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
-        self._spawn_struct = s
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_ROUNDABOUT_GENERIC,
+                                          u=N.HwyNetScenarioUnion(roundabout_generic=s))
 
     def to_finite_mdp(self):
         raise NotImplementedError(f"to_finite_mdp on {self.ENV_ID}")

@@ -26,7 +26,6 @@ def make_two_way_network(length: float = 800) -> NetworkTable:
 
 class BatchedTwoWayEnv(BatchedRoundaboutEnv):
     ENV_ID = "two-way-v0"
-    RESET_ENTRY = "hwy_two_way_reset"
     N_VEHICLES = 6
     EGO_SIDE_LANES = 2  # ("a", "b", 0 / 1)
     REWARD_NAMES = ("high_speed_reward", "left_lane_reward")  # _rewards :50-59
@@ -36,7 +35,7 @@ class BatchedTwoWayEnv(BatchedRoundaboutEnv):
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError("two-way-v0 resets on the device (hwy_two_way_reset)")
+            raise NotImplementedError("two-way-v0 resets on the device")
         cfg = self.config
         for key, default in (("normalize_reward", False), ("duration", float("inf")), ("lane_change_reward", 0.0)):
             cfg.setdefault(key, default)  # AbstractEnv has none of these; TwoWayEnv never truncates
@@ -51,4 +50,4 @@ class BatchedTwoWayEnv(BatchedRoundaboutEnv):
         s.lane_ab1, s.lane_ba0 = self.net.index[("a", "b", 1)], self.net.index[("b", "a", 0)]
         ts = self.action_type.target_speeds
         s.ego_speed_index = speed_to_index(ts, 30.0)
-        self._spawn_struct = s
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_TWO_WAY, u=N.HwyNetScenarioUnion(two_way=s))

@@ -35,7 +35,6 @@ def make_u_turn_network(length: float = 128) -> NetworkTable:
 
 class BatchedUTurnEnv(BatchedRoundaboutEnv):
     ENV_ID = "u-turn-v0"
-    RESET_ENTRY = "hwy_u_turn_reset"
     N_VEHICLES = 7
     EGO_SIDE_LANES = 2  # ("a", "b", 0 / 1)
     REWARD_NAMES = ("collision_reward", "left_lane_reward", "high_speed_reward", "on_road_reward")  # _rewards :61-72
@@ -48,7 +47,7 @@ class BatchedUTurnEnv(BatchedRoundaboutEnv):
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
-            raise NotImplementedError("u-turn-v0 resets on the device (hwy_u_turn_reset)")
+            raise NotImplementedError("u-turn-v0 resets on the device")
         cfg = self.config
         cfg.setdefault("lane_change_reward", 0.0)
         super().define_spaces()
@@ -67,7 +66,7 @@ class BatchedUTurnEnv(BatchedRoundaboutEnv):
         ts = self.action_type.target_speeds
         s.ego_speed_index = speed_to_index(ts, 16.0)
         s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
-        self._spawn_struct = s
+        self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_U_TURN, u=N.HwyNetScenarioUnion(u_turn=s))
 
 
 class BatchedConnectedLaneUTurnEnv(BatchedUTurnEnv):

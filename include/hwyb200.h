@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define HWY_ABI_VERSION 16
+#define HWY_ABI_VERSION 17
 #define HWY_MAX_LANES 8
 #define HWY_MAX_TARGET_SPEEDS 8
 #define HWY_MAX_VEHICLES 128 /* per env, incl. the ego */
@@ -347,54 +347,35 @@ typedef struct HwyNetState {
                                   * means the env has left the reference's trajectory (info["spawn_overflow"]) */
 } HwyNetState;
 
-/* IntersectionEnv._spawn_vehicle constants (envs/intersection_env.py:325-352). */
+/* intersection-v0 (HWY_SCENARIO_INTERSECTION, s->vp == HWY_NET_GROUP_LARGE).
+ * Step: RegulatedRoad rules every int(simulation_frequency / 2) substeps, and after the observation the step's
+ * _clear_vehicles and _spawn_vehicle(spawn_probability) drawing from s->rng (IntersectionEnv.step, :136-140), with
+ * these _spawn_vehicle constants (envs/intersection_env.py:325-352).  With config["controlled_vehicles"] =
+ * p->n_agents > 1 (intersection-multi-agent-v0, envs/intersection_env.py:376-420): action [n_envs][n_agents], obs
+ * [n_envs][n_agents][K][F]; reward is the mean of the agents' rewards, terminated = any crashed or all arrived
+ * (:62-134); agents_reward / agents_terminated [n_envs][n_agents] (NULL for a single agent; optional) are _info's
+ * per-agent entries, which MultiAgentWrapper (abstract.py:468-477) returns in place of the scalar reward / terminated.
+ * Reset: IntersectionEnv._reset / _make_vehicles (:119-122,245-323): n-1 _spawn_vehicle draws, 3 s of warm-up
+ * simulation, the challenger, the controlled vehicle (MDPVehicle on ("o0","ir0",0) at 60 + 5*normal(1)), the 20 m
+ * pruning; all draws come from s->rng in the reference's order. */
 typedef struct HwyIntersectionSpawn {
     int32_t spawn_lane[4];      /* table index of ("o"+k, "ir"+k, 0) */
     double spawn_probability;   /* config["spawn_probability"] */
     const int32_t *route_table; /* DEVICE [n_lanes][4][HWY_NET_MAX_ROUTE]: plan_route_to(lane, "o"+k) */
     const int32_t *route_len;   /* DEVICE [n_lanes][4] */
-    /* _make_vehicles (:245-323), used by hwy_intersection_reset */
+    /* _make_vehicles (:245-323), used by the reset */
     int32_t ego_lane;              /* table index of ("o0", "ir0", 0) */
     int32_t ego_destination;       /* k of config["destination"] == "o"+k; -1 (None): "o" + integers(1, 4) */
     int32_t initial_vehicle_count; /* config["initial_vehicle_count"] */
     int32_t _pad;
     int32_t *scratch;              /* DEVICE [2 * (n_envs + 1)] int32: work lists (envs being reset; the
-                                    * step's 16-slot / 32-slot populations).  NULL: hwy_intersection_step
-                                    * runs every env on 32 slots and hwy_intersection_reset is unavailable */
+                                    * step's 16-slot / 32-slot populations).  NULL: the step runs every env
+                                    * on 32 slots and the reset is unavailable */
 } HwyIntersectionSpawn;
 
 /* observation size in floats PER ENV: Kinematics K*F, TimeToCollision 3*3*(horizon*policy_frequency),
  * OccupancyGrid 4*11*11; times n_agents when several vehicles are controlled */
 int hwy_network_obs_size(const HwyNetParams *p);
-
-/* AbstractEnv.step (abstract.py:259-285) on a general network: action [n_envs] int32
- * (DiscreteMetaAction labels, action.py:204).  graph is a DEVICE pointer. */
-int hwy_network_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetState *s,
-                     const int32_t *action, float *obs, double *reward, uint8_t *terminated,
-                     uint8_t *truncated, double *info_speed, uint8_t *info_crashed, void *stream);
-
-/* Same for intersection-v0 (s->vp == HWY_NET_GROUP_LARGE): RegulatedRoad rules every
- * int(simulation_frequency / 2) substeps, and after the observation the step's _clear_vehicles and
- * _spawn_vehicle(spawn_probability) drawing from s->rng (IntersectionEnv.step, :136-140).
- * With config["controlled_vehicles"] = p->n_agents > 1 (intersection-multi-agent-v0,
- * envs/intersection_env.py:376-420): action [n_envs][n_agents], obs [n_envs][n_agents][K][F]; reward is the mean
- * of the agents' rewards, terminated = any crashed or all arrived (:62-134); agents_reward / agents_terminated
- * [n_envs][n_agents] (NULL for a single agent; optional) are _info's per-agent entries, which MultiAgentWrapper
- * (abstract.py:468-477) returns in place of the scalar reward / terminated. */
-int hwy_intersection_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyIntersectionSpawn *spawn,
-                          const HwyNetState *s, const int32_t *action, float *obs, double *reward,
-                          uint8_t *terminated, uint8_t *truncated, double *info_speed,
-                          uint8_t *info_crashed, double *agents_reward, uint8_t *agents_terminated,
-                          void *stream);
-
-/* IntersectionEnv._reset / _make_vehicles (envs/intersection_env.py:119-122,245-323) on the device for the
- * envs with mask_a[e] | mask_b[e] (both NULL: every env): n-1 _spawn_vehicle draws, 3 s of warm-up simulation,
- * the challenger, the controlled vehicle (MDPVehicle on ("o0","ir0",0) at 60 + 5*normal(1)), the 20 m pruning;
- * all draws come from s->rng in the reference's order.  With final_obs, obs is first copied there (the
- * SameStep autoreset's info["final_obs"]); the fresh observation of the reset envs is written to obs. */
-int hwy_intersection_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyIntersectionSpawn *spawn,
-                           const HwyNetState *s, const uint8_t *mask_a, const uint8_t *mask_b, float *obs,
-                           float *final_obs, void *stream);
 
 /* Test entries (the reference's own known-answer tests run against the device functions):
  * Road.neighbour_vehicles(v, lane) (road/road.py:483-547) for every vehicle v of every env — lane = query_lane
@@ -459,35 +440,28 @@ enum {
 int hwy_debug_pcg64(int op, int arg_i, double arg_lo, double arg_hi, int count, const uint64_t *words_in,
                     uint64_t *words_out, uint64_t *draws, int n, void *stream);
 
-/* Road.act() + Road.step(dt) n_substeps times without an ego action, for the envs whose mask byte is
- * set (NULL: all): the 3 s warm-up of IntersectionEnv._make_vehicles (:271-278). */
-int hwy_network_substeps(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetState *s,
-                         const uint8_t *mask, int n_substeps, void *stream);
-
 /* observation_type.observe() of the current state */
 int hwy_network_observe(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetState *s,
                         float *obs, void *stream);
 
-/* MergeEnv._make_vehicles + the Obstacle of _make_road (envs/merge_env.py:150-190) on the device: the MDPVehicle on
- * ("a","b",1) at s = 30, speed 30; three IDM vehicles on ("a","b", integers(2)) at position + uniform(-5, 5) with
- * speed + uniform(-1, 1); the merging vehicle on ("j","k",0) at s = 110, speed 20, target speed 30; and, in the
- * slot after the vehicles, the Obstacle (kind HWY_KIND_OBSTACLE) at the end of the ramp.  mask_a | mask_b select
- * the envs (both NULL: all); with obs, the fresh observation of those envs is written. */
+/* merge-v0 (HWY_SCENARIO_MERGE): MergeEnv._make_vehicles + the Obstacle of _make_road (envs/merge_env.py:150-190)
+ * on the device: the MDPVehicle on ("a","b",1) at s = 30, speed 30; three IDM vehicles on ("a","b", integers(2)) at
+ * position + uniform(-5, 5) with speed + uniform(-1, 1); the merging vehicle on ("j","k",0) at s = 110, speed 20,
+ * target speed 30; and, in the slot after the vehicles, the Obstacle (kind HWY_KIND_OBSTACLE) at the end of the
+ * ramp. */
 typedef struct HwyMergeSpawn {
     int32_t lane_ab[2];      /* table indices of ("a","b",0), ("a","b",1) */
     int32_t lane_jk;         /* ("j","k",0) */
     int32_t ego_speed_index; /* MDPVehicle.speed_to_index(30) */
     double obstacle_x, obstacle_y;
 } HwyMergeSpawn;
-int hwy_merge_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyMergeSpawn *spawn,
-                    const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
-                    float *obs, void *stream);
 
-/* UTurnEnv._make_vehicles (envs/u_turn_env.py:179-275) on the device: the MDPVehicle at the start of ("a","b",0),
- * speed 16, and six IDM vehicles made with make_on_lane(lane[v], longitudinal[v] + 2 normal(), speed[v] + 2 normal());
- * vehicle 1 also draws its DELTA (randomize_behavior); every vehicle gets plan_route_to("d") from a host-built
- * table indexed by the closest lane.  (The reference also sets ego.PURSUIT_TAU, an attribute nothing reads —
- * steering_control uses TAU_PURSUIT, vehicle/controller.py:28,159 — so there is nothing to restate.) */
+/* u-turn-v0 (HWY_SCENARIO_U_TURN): UTurnEnv._make_vehicles (envs/u_turn_env.py:179-275) on the device: the
+ * MDPVehicle at the start of ("a","b",0), speed 16, and six IDM vehicles made with make_on_lane(lane[v],
+ * longitudinal[v] + 2 normal(), speed[v] + 2 normal()); vehicle 1 also draws its DELTA (randomize_behavior); every
+ * vehicle gets plan_route_to("d") from a host-built table indexed by the closest lane.  (The reference also sets
+ * ego.PURSUIT_TAU, an attribute nothing reads — steering_control uses TAU_PURSUIT, vehicle/controller.py:28,159 — so
+ * there is nothing to restate.) */
 typedef struct HwyUTurnSpawn {
     int32_t lane[8];             /* [0] ego lane ("a","b",0); [1..6] make_on_lane lanes */
     double longitudinal[8], speed[8];
@@ -495,14 +469,12 @@ typedef struct HwyUTurnSpawn {
     const int32_t *route_table;  /* DEVICE [n_lanes][HWY_NET_MAX_ROUTE]: plan_route_to("d") from each lane */
     const int32_t *route_len;    /* DEVICE [n_lanes] */
 } HwyUTurnSpawn;
-int hwy_u_turn_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyUTurnSpawn *spawn,
-                     const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
-                     float *obs, void *stream);
 
-/* ExitEnv._create_vehicles (envs/exit_env.py:107-145) on the device: the MDPVehicle from Vehicle.create_random(speed=25,
- * lane ("0","1",0), spacing=ego_spacing); vehicles_count IDMVehicles on ("0","1", choice(lanes, p=lanes/sum)) at the
- * lane's speed limit, spacing 1 / vehicles_density, routed to "3", enable_lane_change=False.  State stride 32, s->count
- * is set to n_vehicles. */
+/* exit-v0 (HWY_SCENARIO_EXIT): ExitEnv._create_vehicles (envs/exit_env.py:107-145) on the device: the MDPVehicle from
+ * Vehicle.create_random(speed=25, lane ("0","1",0), spacing=ego_spacing); vehicles_count IDMVehicles on ("0","1",
+ * choice(lanes, p=lanes/sum)) at the lane's speed limit, spacing 1 / vehicles_density, routed to "3",
+ * enable_lane_change=False.  State stride 32, s->count is set to n_vehicles.  The step is the 32-slot one without
+ * rules or population changes. */
 typedef struct HwyExitSpawn {
     int32_t lanes_count, n_vehicles;   /* config["lanes_count"], 1 + config["vehicles_count"] */
     int32_t ego_speed_index, _pad;
@@ -511,24 +483,20 @@ typedef struct HwyExitSpawn {
     double cdf[HWY_MAX_LANES];         /* Generator.choice(p=lanes / lanes.sum()): p.cumsum() / cumsum[-1] */
     int32_t route_12, route_23;        /* encoded route entries ("1","2",None), ("2","3",None) */
 } HwyExitSpawn;
-int hwy_exit_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyExitSpawn *spawn, const HwyNetState *s,
-                   uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b, float *obs, void *stream);
 
-/* TwoWayEnv._make_vehicles (envs/two_way_env.py:113-158) on the device: the MDPVehicle on ("a","b",1) at s = 30,
- * three IDM vehicles ahead at 70 + 40 i + 10 normal() with speed 24 + 2 normal(), two oncoming ones on ("b","a",0)
- * at 200 + 100 i + 10 normal() with speed 20 + 5 normal(); all traffic has enable_lane_change=False. */
+/* two-way-v0 (HWY_SCENARIO_TWO_WAY): TwoWayEnv._make_vehicles (envs/two_way_env.py:113-158) on the device: the
+ * MDPVehicle on ("a","b",1) at s = 30, three IDM vehicles ahead at 70 + 40 i + 10 normal() with speed 24 + 2 normal(),
+ * two oncoming ones on ("b","a",0) at 200 + 100 i + 10 normal() with speed 20 + 5 normal(); all traffic has
+ * enable_lane_change=False. */
 typedef struct HwyTwoWaySpawn {
     int32_t lane_ab1, lane_ba0; /* table indices of ("a","b",1) and ("b","a",0) */
     int32_t ego_speed_index, _pad;
 } HwyTwoWaySpawn;
-int hwy_two_way_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyTwoWaySpawn *spawn,
-                      const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
-                      float *obs, void *stream);
 
-/* RoundaboutEnv._make_vehicles (envs/roundabout_env.py:317-391) on the device.  Per traffic
- * vehicle the env's numpy stream yields normal (longitudinal), normal (speed),
- * choice(destinations), uniform (DELTA); routes come from a host-built table of
- * ControlledVehicle.plan_route_to results (vehicle/controller.py:71-87). */
+/* roundabout-v0 (HWY_SCENARIO_ROUNDABOUT): RoundaboutEnv._make_vehicles (envs/roundabout_env.py:317-391) on the
+ * device.  Per traffic vehicle the env's numpy stream yields normal (longitudinal), normal (speed),
+ * choice(destinations), uniform (DELTA); routes come from a host-built table of ControlledVehicle.plan_route_to
+ * results (vehicle/controller.py:71-87). */
 typedef struct HwyRoundaboutSpawn {
     int32_t ego_lane;            /* table index of ("ser", "ses", 0) */
     int32_t spawn_lane[4];       /* make_on_lane lanes: (we,sx,1), (we,sx,0), (we,sx,0), (eer,ees,0) */
@@ -543,20 +511,14 @@ typedef struct HwyRoundaboutSpawn {
     const int32_t *route_len;    /* DEVICE [n_lanes][4] */
 } HwyRoundaboutSpawn;
 
-/* Re-spawn the envs selected by mask_a | mask_b (both NULL: all) from rng[5*n_envs] (layout as
- * HwyHighwayState.rng); if obs != NULL also write their reset observation. */
-int hwy_roundabout_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyRoundaboutSpawn *spawn,
-                         const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
-                         float *obs, void *stream);
-
-/* RoundaboutGenericEnv._make_vehicles (envs/roundabout_env.py:664-751; roundabout-generic-v0 / v1) on the device:
- * the MDPVehicle at length - 2.5 of ("ser","ses",0), speed 8, routed to "nxs"; then for each of vehicles_count
- * vehicles up to 10 tries of integers(0, 7) (spawn road), integers(0, lanes of the road) (no draw on a one-lane
- * road), uniform(5, max(5, length - 5)) (longitudinal), rejected when the point lies closer than 7 m to a point
- * already placed; an accepted try draws its speed 14 + 2 normal(), its destination integers(0, 4) (none when
- * fixed_destination >= 0) and DELTA uniform(3.5, 4.5), and plans its route from its closest lane.  A vehicle whose
- * 10 tries all fail is skipped: s->count (required) receives the population and the slots past it are cleared.
- * Slot stride 8 or 32. */
+/* roundabout-generic-v0 / v1 (HWY_SCENARIO_ROUNDABOUT_GENERIC): RoundaboutGenericEnv._make_vehicles
+ * (envs/roundabout_env.py:664-751) on the device: the MDPVehicle at length - 2.5 of ("ser","ses",0), speed 8, routed
+ * to "nxs"; then for each of vehicles_count vehicles up to 10 tries of integers(0, 7) (spawn road), integers(0, lanes
+ * of the road) (no draw on a one-lane road), uniform(5, max(5, length - 5)) (longitudinal), rejected when the point
+ * lies closer than 7 m to a point already placed; an accepted try draws its speed 14 + 2 normal(), its destination
+ * integers(0, 4) (none when fixed_destination >= 0) and DELTA uniform(3.5, 4.5), and plans its route from its closest
+ * lane.  A vehicle whose 10 tries all fail is skipped: s->count (required) receives the population and the slots past
+ * it are cleared.  Slot stride 8 or 32; on 32 slots the step is the one without rules or population changes. */
 typedef struct HwyRoundaboutGenericSpawn {
     int32_t ego_lane;            /* table index of ("ser", "ses", 0) */
     int32_t spawn_road[7];       /* table index of lane 0 of (we,sx), (sx,se), (ee,nx), (nx,ne), (eer,ees), (ner,nes),
@@ -569,15 +531,19 @@ typedef struct HwyRoundaboutGenericSpawn {
                                   * nxr, wxr; 4 = the ego's nxs */
     const int32_t *route_len;    /* DEVICE [n_lanes][route_width] */
 } HwyRoundaboutGenericSpawn;
-int hwy_roundabout_generic_reset(const HwyNetParams *p, const HwyNetGraph *graph,
-                                 const HwyRoundaboutGenericSpawn *spawn, const HwyNetState *s, uint64_t *rng,
-                                 const uint8_t *mask_a, const uint8_t *mask_b, float *obs, void *stream);
 
-/* RacetrackEnv (envs/racetrack_env.py:15-425; racetrack-v0, and racetrack-v1 with connected_lanes) and its large
- * (RacetrackEnvLarge, :432-880) and oval (RacetrackEnvOval, :882-1396) tracks on the 8-slot network state, which must carry s->count (the population: the ego, the front vehicle and the extra vehicles that
- * survived the 20 m check).  The controlled vehicle is a plain Vehicle (HWY_KIND_VEHICLE) in slot 0 whose (target_speed,
- * timer) pair holds its persisting action dict (acceleration, steering) (vehicle/kinematics.py:119-128); `action` is
- * float32 [n_envs][2] = (throttle, steering) as passed, a missing control axis staged as 0 with the range (0, 0) in p. */
+/* racetrack-v0 / v1 and racetrack-large / racetrack-oval (HWY_SCENARIO_RACETRACK): RacetrackEnv
+ * (envs/racetrack_env.py:15-425; v1 with connected_lanes) and its large (RacetrackEnvLarge, :432-880) and oval
+ * (RacetrackEnvOval, :882-1396) tracks on the 8-slot network state, which must carry s->count (the population: the
+ * ego, the front vehicle and the extra vehicles that survived the 20 m check).  The controlled vehicle is a plain
+ * Vehicle (HWY_KIND_VEHICLE) in slot 0 whose (target_speed, timer) pair holds its persisting action dict
+ * (acceleration, steering) (vehicle/kinematics.py:119-128); `action` is float32 [n_envs][2] = (throttle, steering) as
+ * passed, a missing control axis staged as 0 with the range (0, 0) in p.
+ * Reset: _make_vehicles (:374-425), drawing from s->rng in the reference's order; slots past the population are
+ * cleared.  Step: one RacetrackEnv.step of every env — the action, simulation_frequency / policy_frequency substeps,
+ * observation, reward (:66-83; s->reward_terms: lane_centering, action, collision, on_road), terminated (crashed, or
+ * off road with terminate_off_road), truncated (time >= duration).  Substeps: Road.act + Road.step with the
+ * persisting action, on every env. */
 typedef struct HwyRacetrackParams {
     int32_t other_vehicles;      /* config["other_vehicles"], 0..HWY_NET_GROUP - 1 */
     int32_t terminate_off_road;  /* config["terminate_off_road"] */
@@ -587,19 +553,51 @@ typedef struct HwyRacetrackParams {
                                   * at most the lane count of ("a","b") and of ("b","c"), which the caller checks */
     double lane_centering_cost, lane_centering_reward, action_reward, collision_reward, on_road_reward;
 } HwyRacetrackParams;
-/* _make_vehicles (:374-425) for the envs selected by mask_a | mask_b (both NULL: all), drawing from rng[5*n_envs] in
- * the reference's order; slots past the population are cleared.  obs != NULL: also their reset observation. */
-int hwy_racetrack_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyRacetrackParams *rp,
-                        const HwyNetState *s, uint64_t *rng, const uint8_t *mask_a, const uint8_t *mask_b,
-                        float *obs, void *stream);
-/* n_substeps == 0: one RacetrackEnv.step of every env — the action, simulation_frequency / policy_frequency substeps,
- * observation, reward (:66-83; s->reward_terms: lane_centering, action, collision, on_road), terminated (crashed, or
- * off road with terminate_off_road), truncated (time >= duration).  n_substeps > 0: that many Road.act + Road.step
- * with the persisting action and nothing else; action and the outputs are then not read or written (may be NULL). */
-int hwy_racetrack_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyRacetrackParams *rp,
-                       const HwyNetState *s, const float *action, int n_substeps, float *obs, double *reward,
-                       uint8_t *terminated, uint8_t *truncated, double *info_speed, uint8_t *info_crashed,
-                       void *stream);
+
+/* The scenario of a network entry point: `kind` names the union member the entry reads.  HWY_SCENARIO_NONE (or a NULL
+ * scenario where one is optional) reads none: the step and the substeps then run the plain network kernels. */
+enum {
+    HWY_SCENARIO_NONE = 0, HWY_SCENARIO_ROUNDABOUT, HWY_SCENARIO_ROUNDABOUT_GENERIC, HWY_SCENARIO_MERGE,
+    HWY_SCENARIO_TWO_WAY, HWY_SCENARIO_U_TURN, HWY_SCENARIO_EXIT, HWY_SCENARIO_INTERSECTION, HWY_SCENARIO_RACETRACK
+};
+typedef struct HwyNetScenario {
+    int32_t kind, _pad; /* HWY_SCENARIO_* */
+    union {
+        HwyRoundaboutSpawn roundabout;
+        HwyRoundaboutGenericSpawn roundabout_generic;
+        HwyMergeSpawn merge;
+        HwyTwoWaySpawn two_way;
+        HwyUTurnSpawn u_turn;
+        HwyExitSpawn exit;
+        HwyIntersectionSpawn intersection;
+        HwyRacetrackParams racetrack;
+    } u;
+} HwyNetScenario;
+
+/* AbstractEnv.reset()'s _reset() of scenario sc (required, not NONE) for the envs with mask_a[e] | mask_b[e] (both
+ * NULL: every env), drawing from s->rng (required).  With final_obs, obs is first copied there (the SameStep
+ * autoreset's info["final_obs"]); with obs, the fresh observation of the reset envs is written to obs. */
+int hwy_network_reset(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetScenario *sc, const HwyNetState *s,
+                      const uint8_t *mask_a, const uint8_t *mask_b, float *obs, float *final_obs, void *stream);
+
+/* AbstractEnv.step (abstract.py:259-285) of every env on a general network.  graph is a DEVICE pointer; sc may be
+ * NULL (kind NONE).  action: int32 DiscreteMetaAction labels (action.py:204), [n_envs] or [n_envs][n_agents]; float32
+ * [n_envs][2] (throttle, steering) when p->action_type == 1.  obs [n_envs][hwy_network_obs_size] f32, reward [n_envs]
+ * f64, terminated / truncated [n_envs] u8; info_speed [n_envs] f64 / info_crashed [n_envs] u8 (either may be NULL);
+ * agents_reward / agents_terminated: see HwyIntersectionSpawn.  Kind RACETRACK runs the racetrack step; every other
+ * kind runs on the slot stride: 8 slots the roundabout family's step, 32 slots the intersection family's, with the
+ * rules, population changes and 16 / 32-slot split of kind INTERSECTION, without them for any other kind. */
+int hwy_network_step(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetScenario *sc, const HwyNetState *s,
+                     const void *action, float *obs, double *reward, uint8_t *terminated, uint8_t *truncated,
+                     double *info_speed, uint8_t *info_crashed, double *agents_reward, uint8_t *agents_terminated,
+                     void *stream);
+
+/* Road.act() + Road.step(dt) n_substeps times without an ego action, and nothing else, for the envs whose mask byte
+ * is set (NULL: all): the 3 s warm-up of IntersectionEnv._make_vehicles (:271-278), and env.road_substeps.  sc may be
+ * NULL (kind NONE).  Kind RACETRACK runs every env (mask must be NULL), its plain ego keeping its persisting action;
+ * there n_substeps == 0 launches nothing. */
+int hwy_network_substeps(const HwyNetParams *p, const HwyNetGraph *graph, const HwyNetScenario *sc,
+                         const HwyNetState *s, const uint8_t *mask, int n_substeps, void *stream);
 
 /* ====================================================================== observation plugins on ANY road family
  * The reference's observation_factory (envs/common/observation.py:772-794) builds any ObservationType on any env; these

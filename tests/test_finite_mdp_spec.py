@@ -20,7 +20,7 @@ def test_planner_entries_are_exported():
     for sym in ("hwy_finite_mdp", "hwy_value_iteration"):
         assert sym in N.EXPORTS
         assert getattr(lib, sym) is not None
-    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 16
+    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 17
 
 
 def test_planner_structs_match_gcc():

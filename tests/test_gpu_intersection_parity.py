@@ -151,7 +151,7 @@ def test_free_running_rollout_and_autoreset():
 
 @pytest.mark.parametrize("name", CASES)
 def test_device_reset_matches_host_reset(name):
-    """hwy_intersection_reset (all of _make_vehicles in one kernel) against the numpy-exact host sequence:
+    """The intersection reset (all of _make_vehicles in one kernel) against the numpy-exact host sequence:
     the same draws word for word, the same population, lanes and routes; coordinates within the rounding
     of CUDA-vs-numpy sin/cos carried through the 45 warm-up substeps."""
     g = load_golden(name)
@@ -201,7 +201,7 @@ def test_device_autoreset_masks_only_finished_envs():
 
 
 def test_16_slot_and_32_slot_paths_agree():
-    """hwy_intersection_step runs populations of <= 15 vehicles two per warp on 16 slots and the others on 32
+    """The intersection step runs populations of <= 15 vehicles two per warp on 16 slots and the others on 32
     (work lists in spawn.scratch); without scratch every env takes the 32-slot kernel.  Same results bit for bit."""
     g = load_golden("intersection_grid")
     n = 256

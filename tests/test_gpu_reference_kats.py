@@ -197,7 +197,7 @@ def test_road_network_follow_road():
     p.distance_wanted, p.time_wanted, p.lane_change_delay = 10.0, 1.5, 1.0
     lane, changes = 0, 0
     for _ in range(20 * 15):
-        N.check(lib.hwy_network_substeps(C.byref(p), graph.data_ptr(), C.byref(st), None, 1, None))
+        N.check(lib.hwy_network_substeps(C.byref(p), graph.data_ptr(), None, C.byref(st), None, 1, None))
         tgt = (int(meta[1, 0]) >> N.META_TARGET_SHIFT) & 0xFF
         if tgt != lane:
             lane, changes = tgt, changes + 1
@@ -274,7 +274,7 @@ def _single_lane_device(x, speed, kinds):
 def test_behavior_stop_before_obstacle():
     """vehicle/test_behavior.py:13-27 on the device"""
     N, p, graph, st, t = _single_lane_device([0.0, 80.0], [20.0, 0.0], [0, 3])
-    N.check(N.load().hwy_network_substeps(C.byref(p), graph.data_ptr(), C.byref(st), None, 10 * K.FPS, None))
+    N.check(N.load().hwy_network_substeps(C.byref(p), graph.data_ptr(), None, C.byref(st), None, 10 * K.FPS, None))
     torch.cuda.synchronize()
     x, y = float(t["pos"][1, 0, 0]), float(t["pos"][1, 0, 1])
     assert not (int(t["meta"][1, 0]) & N.META_CRASHED)
@@ -286,6 +286,6 @@ def test_behavior_stop_before_obstacle():
 def test_dynamics_collision_with_obstacle():
     """vehicle/test_dynamics.py:56-60 on the device"""
     N, p, graph, st, t = _single_lane_device([20.0, 23.0], [10.0, 0.0], [0, 3])
-    N.check(N.load().hwy_network_substeps(C.byref(p), graph.data_ptr(), C.byref(st), None, 1, None))
+    N.check(N.load().hwy_network_substeps(C.byref(p), graph.data_ptr(), None, C.byref(st), None, 1, None))
     torch.cuda.synchronize()
     assert int(t["meta"][1, 0]) & N.META_CRASHED and int(t["meta"][1, 1]) & N.META_CRASHED

@@ -29,6 +29,33 @@ def test_library_exports_every_declared_symbol():
     assert lib.hwy_highway_slot_stride(51) == 52 and lib.hwy_highway_slot_stride(20) == 20
 
 
+def test_network_entries_refuse_bad_scenarios_without_gpu():
+    """hwy_network_reset / _step / _substeps refuse an unknown scenario kind, a reset without a scenario or without
+    the rng words, and a mask on the racetrack substeps (which run every env) before any device call."""
+    import ctypes as C
+
+    from highwayenv_b200 import _native as N
+
+    lib = N.load()
+    p, st, sc = N.HwyNetParams(), N.HwyNetState(), N.HwyNetScenario()
+    buf = (C.c_double * 64)()
+    ptr = C.addressof(buf)
+    P, S = C.byref(p), C.byref(st)
+    sc.kind = N.HWY_SCENARIO_RACETRACK + 1
+    for rc in (lib.hwy_network_reset(P, ptr, C.byref(sc), S, None, None, None, None, None),
+               lib.hwy_network_step(P, ptr, C.byref(sc), S, ptr, ptr, ptr, ptr, ptr, None, None, None, None, None),
+               lib.hwy_network_substeps(P, ptr, C.byref(sc), S, None, 1, None)):
+        assert rc != 0 and b"unknown scenario kind" in lib.hwy_last_error()
+    assert lib.hwy_network_reset(P, ptr, None, S, None, None, None, None, None) != 0
+    assert b"null scenario" in lib.hwy_last_error()
+    sc.kind = N.HWY_SCENARIO_ROUNDABOUT
+    assert lib.hwy_network_reset(P, ptr, C.byref(sc), S, None, None, None, None, None) != 0  # st.rng is NULL
+    assert b"null rng" in lib.hwy_last_error()
+    sc.kind = N.HWY_SCENARIO_RACETRACK
+    assert lib.hwy_network_substeps(P, ptr, C.byref(sc), S, ptr, 1, None) != 0
+    assert b"mask must be NULL" in lib.hwy_last_error()
+
+
 def test_struct_layout_matches_header():
     """ctypes mirrors must have the C sizes (gcc as the referee)."""
     import ctypes as C
@@ -36,11 +63,12 @@ def test_struct_layout_matches_header():
 
     from highwayenv_b200 import _native as N
 
-    src = ('#include <stdio.h>\n#include "hwyb200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", '
+    src = ('#include <stdio.h>\n#include <stddef.h>\n#include "hwyb200.h"\nint main(){printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", '
            'sizeof(HwyHighwayParams), sizeof(HwyHighwayState), sizeof(HwyStraightLane), sizeof(HwyNetLane), '
            'sizeof(HwyNetGraph), sizeof(HwyNetParams), sizeof(HwyNetState), sizeof(HwyIntersectionSpawn), '
            'sizeof(HwyRoundaboutSpawn), sizeof(HwyObsView), sizeof(HwyGridParams), sizeof(HwyTtcParams), '
-           'sizeof(HwyLidarParams), sizeof(HwyExitSpawn));return 0;}\n')
+           'sizeof(HwyLidarParams), sizeof(HwyExitSpawn), sizeof(HwyNetScenario), offsetof(HwyNetScenario, u));'
+           'return 0;}\n')
     with tempfile.TemporaryDirectory() as d:
         open(os.path.join(d, "t.c"), "w").write(src)
         exe = os.path.join(d, "t")
@@ -49,7 +77,7 @@ def test_struct_layout_matches_header():
     assert sizes == [C.sizeof(t) for t in (N.HwyHighwayParams, N.HwyHighwayState, N.HwyStraightLane, N.HwyNetLane,
                                            N.HwyNetGraph, N.HwyNetParams, N.HwyNetState, N.HwyIntersectionSpawn,
                                            N.HwyRoundaboutSpawn, N.HwyObsView, N.HwyGridParams, N.HwyTtcParams,
-                                           N.HwyLidarParams, N.HwyExitSpawn)]
+                                           N.HwyLidarParams, N.HwyExitSpawn, N.HwyNetScenario)] + [N.HwyNetScenario.u.offset]
 
 
 def test_abi_validation_without_gpu():

@@ -175,7 +175,7 @@ def test_struct_layout_matches_gcc():
         want += [getattr(t, f).offset for f in names]
     assert got == want
     hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
-    assert "#define HWY_ABI_VERSION 16" in hdr and N.HWY_ABI_VERSION == 16
+    assert "#define HWY_ABI_VERSION 17" in hdr and N.HWY_ABI_VERSION == 17
     assert {"hwy_lane_keeping_reset", "hwy_lane_keeping_step"} <= set(N.EXPORTS)
 
 

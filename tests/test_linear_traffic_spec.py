@@ -146,7 +146,7 @@ def test_linear_entries_and_struct():
                lib.hwy_highway_step(P, S, T, None, None, None, None, None, None, None, None, 0, None, None),
                lib.hwy_highway_substeps(P, S, T, 1, None, None)):
         assert rc != 0 and b"null linear traffic parameters" in lib.hwy_last_error()
-    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 16
+    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 17
     src = ('#include <stdio.h>\n#include <stddef.h>\n#include "hwyb200.h"\nint main(){printf("%zu %zu %zu %zu %zu %d\\n", '
            'sizeof(HwyLinearTraffic), offsetof(HwyLinearTraffic, acc_span), offsetof(HwyLinearTraffic, steer_lo), '
            'offsetof(HwyLinearTraffic, steer_span), offsetof(HwyLinearTraffic, acc_lo), HWY_LINEAR_PARAMS);return 0;}\n')

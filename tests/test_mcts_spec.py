@@ -24,7 +24,7 @@ def test_new_entries_are_exported():
     for sym in NEW_ENTRIES:
         assert sym in N.EXPORTS
         assert getattr(lib, sym) is not None
-    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 16
+    assert lib.hwy_abi_version() == N.HWY_ABI_VERSION == 17
 
 
 def test_tree_struct_matches_gcc():

@@ -166,9 +166,12 @@ def test_struct_layout_matches_gcc():
     want = [C.sizeof(N.HwyRacetrackParams)] + [getattr(N.HwyRacetrackParams, f).offset for f in names]
     assert got == want
     hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
-    assert "#define HWY_ABI_VERSION 16" in hdr and N.HWY_ABI_VERSION == 16
-    for sym in ("hwy_racetrack_reset", "hwy_racetrack_step"):
+    assert "#define HWY_ABI_VERSION 17" in hdr and N.HWY_ABI_VERSION == 17
+    # the racetrack runs on the network entry points with its scenario, not on entry points of its own
+    for sym in ("hwy_network_reset", "hwy_network_step", "hwy_network_substeps"):
         assert sym in N.EXPORTS and sym + "(" in hdr
+    for sym in ("hwy_racetrack_reset", "hwy_racetrack_step"):
+        assert sym not in N.EXPORTS and sym not in hdr, sym
 
 
 def _cfg(**over):

@@ -291,4 +291,11 @@ def test_registered():
                         ("roundabout-generic-v1", "BatchedConnectedLaneRoundaboutGenericEnv")]:
         assert hb.REGISTRY[env_id].endswith(":" + cls)
         assert default_config(env_id)["neighbour_vehicles_connected_lanes"] is env_id.endswith("v1")
-    assert "hwy_roundabout_generic_reset" in N.EXPORTS and N.HWY_ABI_VERSION == 16
+    assert N.HWY_ABI_VERSION == 17
+    # every network scenario resets and steps through the network entry points with its HwyNetScenario
+    hdr = open(os.path.join(ROOT, "include", "hwyb200.h")).read()
+    for sym in ("hwy_network_reset", "hwy_network_step", "hwy_network_substeps"):
+        assert sym in N.EXPORTS and sym + "(" in hdr
+    for sym in ("hwy_roundabout_generic_reset", "hwy_roundabout_reset", "hwy_merge_reset", "hwy_two_way_reset",
+                "hwy_u_turn_reset", "hwy_exit_reset", "hwy_intersection_reset", "hwy_intersection_step"):
+        assert sym not in N.EXPORTS and sym not in hdr, sym
