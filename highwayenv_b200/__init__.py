@@ -39,6 +39,9 @@ REGISTRY = {
     "exit-v1": "highwayenv_b200.envs.exit_env:BatchedConnectedLaneExitEnv",
     "merge-v0": "highwayenv_b200.envs.merge_env:BatchedMergeEnv",
     "merge-v1": "highwayenv_b200.envs.merge_env:BatchedConnectedLaneMergeEnv",
+    # the merge of config["lanes_count"] lanes and four section lengths with vehicles_count rejection-sampled cars
+    "merge-generic-v0": "highwayenv_b200.envs.merge_env:BatchedMergeGenericEnv",
+    "merge-generic-v1": "highwayenv_b200.envs.merge_env:BatchedConnectedLaneMergeGenericEnv",
     # MultiAgentAction / MultiAgentObservation (v1, v2: behind MultiAgentWrapper)
     "intersection-multi-agent-v0": "highwayenv_b200.envs.intersection_env:BatchedMultiAgentIntersectionEnv",
     "intersection-multi-agent-v1": "highwayenv_b200.envs.intersection_env:BatchedMultiAgentWrappedIntersectionEnv",

@@ -125,7 +125,7 @@ class HwyNetParams(C.Structure):
                                     "dynamic_population", "connected_lanes", "n_agents")]
         + [(n, C.c_double) for n in ("arrived_reward", "reward_speed_lo", "reward_speed_hi", "right_lane_reward",
                                      "merging_speed_reward")]
-        + [("merge_lane", C.c_int32), ("_pad_merge", C.c_int32), ("left_lane_reward", C.c_double),
+        + [("merge_lane", C.c_int32), ("merge_end_lane", C.c_int32), ("left_lane_reward", C.c_double),
            ("goal_reward", C.c_double), ("exit_lane_a", C.c_int32), ("exit_lane_b", C.c_int32),
            ("obs_exit_lane", C.c_int32), ("_pad_exit", C.c_int32),
            ("action_type", C.c_int32), ("act_clip", C.c_int32), ("dynamical", C.c_int32), ("obs_n_feat", C.c_int32),
@@ -154,7 +154,8 @@ class HwyIntersectionSpawn(C.Structure):
 
 class HwyMergeSpawn(C.Structure):
     _fields_ = [("lane_ab", C.c_int32 * 2), ("lane_jk", C.c_int32), ("ego_speed_index", C.c_int32),
-                ("obstacle_x", C.c_double), ("obstacle_y", C.c_double)]
+                ("obstacle_x", C.c_double), ("obstacle_y", C.c_double),
+                ("lanes_count", C.c_int32), ("vehicles_count", C.c_int32), ("max_position", C.c_double)]
 
 
 KIND_OBSTACLE = 3

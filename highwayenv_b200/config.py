@@ -238,6 +238,18 @@ DEFAULTS["merge-v0"] = merge_default_config
 DEFAULTS["merge-v1"] = _connected(merge_default_config)
 
 
+def merge_generic_default_config() -> dict:
+    """MergeGenericEnv.default_config (highway_env/envs/merge_env.py:217-236)."""
+    config = merge_default_config()
+    update_config(config, {"lanes_count": 2, "vehicles_count": 3, "before_merge_length": 150,
+                           "converge_merge_length": 80, "parallel_merge_length": 80, "after_merge_length": 150})
+    return config
+
+
+DEFAULTS["merge-generic-v0"] = merge_generic_default_config
+DEFAULTS["merge-generic-v1"] = _connected(merge_generic_default_config)
+
+
 def two_way_default_config() -> dict:
     """TwoWayEnv.default_config (highway_env/envs/two_way_env.py:17-33) over AbstractEnv's."""
     config = abstract_default_config()

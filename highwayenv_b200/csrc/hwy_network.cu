@@ -1603,7 +1603,8 @@ network_step_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* _
             rt[3] = on_road ? 1.0 : 0.0;
         } else if (P.reward_type == 2) {
             // envs/merge_env.py:39-84: unclipped speed term, lane id of the CURRENT lane, altruistic penalty over the
-            // ControlledVehicles on the merging lane ("b", "c", 2); never truncated, terminated past x = 370
+            // ControlledVehicles on the merging lane ("b", "c", 2); never truncated, terminated past x = 370 or, for
+            // MergeGenericEnv (:249,370-372), past end_position = the end x of a ("c","d") lane - 90
             double scaled_speed = lmap(r.speed, P.reward_speed_lo, P.reward_speed_hi, 0.0, 1.0);
             double merging = 0.0;
             for (int v = 0; v < V; ++v)
@@ -1616,7 +1617,7 @@ network_step_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* _
             rew = rew + P.merging_speed_reward * merging;
             rew = lmap(rew, P.collision_reward + P.merging_speed_reward, P.high_speed_reward + P.right_lane_reward, 0.0,
                        1.0);
-            term = is_crashed || r.x > 370;
+            term = is_crashed || r.x > (P.merge_end_lane > 0 ? g.lanes[P.merge_end_lane].ex - 90.0 : 370.0);
             rt[0] = is_crashed ? 1.0 : 0.0;
             rt[1] = (double)L.lane_id / 1.0;
             rt[2] = scaled_speed;
@@ -2027,6 +2028,31 @@ __device__ __forceinline__ int closest_lane(const HwyNetGraph* graph, double x, 
     return lane;
 }
 
+// The same search by a whole warp (the device resets that give an env one warp): lane l of the table on warp lane
+// l % 32, then a (distance, index) minimum over the warp = np.argmin's first minimum.  Every lane of the warp calls it
+// with the same point and receives the same lane.
+__device__ __forceinline__ int warp_closest_lane(const HwyNetGraph* graph, double px, double py, double heading, int wl) {
+    double bd = INFINITY;
+    int lane = 0x7fffffff;
+    for (int l = wl; l < graph->n_lanes; l += 32) {
+        const double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
+        if (lane == 0x7fffffff || d < bd) {
+            bd = d;
+            lane = l;
+        }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        const double d2 = __shfl_xor_sync(0xffffffffu, bd, off);
+        const int l2 = __shfl_xor_sync(0xffffffffu, lane, off);
+        if (l2 != 0x7fffffff && (lane == 0x7fffffff || d2 < bd || (d2 == bd && l2 < lane))) {
+            bd = d2;
+            lane = l2;
+        }
+    }
+    return lane;
+}
+
 // One placed vehicle into slot k, with no impact; IDM vehicles get IDMVehicle.__init__'s lane-change timer
 // (behavior.py:64).  `flags`: further meta bits (HWY_META_NO_LANE_CHANGE).
 __device__ __forceinline__ void store_vehicle(const HwyNetParams& P, const HwyNetState& S, size_t k, double px,
@@ -2051,6 +2077,20 @@ __device__ __forceinline__ void store_env_tail(const HwyNetState& S, uint64_t* r
     if (S.count) S.count[e] = count;
     if (S.road_steps) S.road_steps[e] = 0;
     store_rng(rng, (size_t)S.n_envs, e, g);
+}
+
+// The slots past a varying population (n vehicles placed), cleared by the env's warp
+__device__ __forceinline__ void clear_slots_past(const HwyNetState& S, size_t base, int n, int wl) {
+    for (int v = n + wl; v < S.vp; v += 32) {
+        const size_t k = base + v;
+        reinterpret_cast<double2*>(S.pos)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.hs)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.tt)[k] = make_double2(0.0, 0.0);
+        reinterpret_cast<double2*>(S.imp)[k] = make_double2(0.0, 0.0);
+        S.delta[k] = 0.0;
+        S.meta[k] = 0;
+        S.route_len[k] = 0;
+    }
 }
 
 // RoundaboutEnv._make_vehicles (envs/roundabout_env.py:317-391), one env per WARP.  The draws are a sequential chain
@@ -2087,25 +2127,7 @@ roundabout_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGrap
             lane_position(L, lon, 0.0, px, py);  // make_on_lane (vehicle/objects.py:68-90)
             heading = lane_heading_at(L, lon);
         }
-        // closest_lane over the warp
-        double bd = INFINITY;
-        int lane = 0x7fffffff;
-        for (int l = wl; l < graph->n_lanes; l += 32) {
-            const double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
-            if (lane == 0x7fffffff || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            const double d2 = __shfl_xor_sync(0xffffffffu, bd, off);
-            const int l2 = __shfl_xor_sync(0xffffffffu, lane, off);
-            if (l2 != 0x7fffffff && (lane == 0x7fffffff || d2 < bd || (d2 == bd && l2 < lane))) {
-                bd = d2;
-                lane = l2;
-            }
-        }
+        const int lane = warp_closest_lane(graph, px, py, heading, wl);
         if (wl == 0) {
             store_vehicle(P, S, base + v, px, py, heading, speed, is_ego ? P.target_speeds[SP.ego_speed_index] : speed,
                           delta, lane, lane, is_ego ? HWY_KIND_MDP : HWY_KIND_IDM);
@@ -2477,24 +2499,7 @@ roundabout_generic_reset_kernel(const __grid_constant__ HwyNetParams P, const Hw
     auto place = [&](const HwyNetLane& L, double lon, double px, double py, double speed, double target_speed,
                      double delta, int dest, int kind) {
         const double heading = lane_heading_at(L, lon);
-        double bd = INFINITY;
-        int lane = 0x7fffffff;
-        for (int l = wl; l < graph->n_lanes; l += 32) {
-            const double d = lane_distance_with_heading(graph->lanes[l], px, py, heading);
-            if (lane == 0x7fffffff || d < bd) {
-                bd = d;
-                lane = l;
-            }
-        }
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) {
-            const double d2 = __shfl_xor_sync(0xffffffffu, bd, off);
-            const int l2 = __shfl_xor_sync(0xffffffffu, lane, off);
-            if (l2 != 0x7fffffff && (lane == 0x7fffffff || d2 < bd || (d2 == bd && l2 < lane))) {
-                bd = d2;
-                lane = l2;
-            }
-        }
+        const int lane = warp_closest_lane(graph, px, py, heading, wl);
         const size_t k = (size_t)lane * SP.route_width + dest;
         if (wl == 0) {
             store_vehicle(P, S, base + n, px, py, heading, speed, target_speed, delta, lane, lane, kind);
@@ -2535,16 +2540,74 @@ roundabout_generic_reset_kernel(const __grid_constant__ HwyNetParams P, const Hw
             break;
         }
     }
-    for (int v = n + wl; v < S.vp; v += 32) {
-        const size_t k = base + v;
-        reinterpret_cast<double2*>(S.pos)[k] = make_double2(0.0, 0.0);
-        reinterpret_cast<double2*>(S.hs)[k] = make_double2(0.0, 0.0);
-        reinterpret_cast<double2*>(S.tt)[k] = make_double2(0.0, 0.0);
-        reinterpret_cast<double2*>(S.imp)[k] = make_double2(0.0, 0.0);
-        S.delta[k] = 0.0;
-        S.meta[k] = 0;
-        S.route_len[k] = 0;
+    clear_slots_past(S, base, n, wl);
+    if (wl == 0) store_env_tail(S, rng, e, SP.ego_speed_index, n, g);
+}
+
+// ------------------------------------------------------------------ merge-generic-v0 / v1 (envs/merge_env.py)
+// MergeGenericEnv._make_vehicles (:320-368) and the Obstacle of _make_road (:317), one env per WARP as
+// roundabout_generic_reset_kernel: every lane of the warp walks the env's draw chain redundantly, and each placed
+// object's closest-lane search at heading 0 is spread over the warp.  spawned_positions is the list of placed (lane id,
+// longitudinal) pairs, at most 30 (the ego and 29 traffic vehicles).  A vehicle whose 10 tries all land within 15 m of
+// a longitudinal already placed on the drawn lane id is skipped, so the population, and with it the Obstacle's slot
+// (count - 1), varies per env; S.count receives the population and the slots past it are cleared.
+__global__ void __launch_bounds__(128)
+merge_generic_reset_kernel(const __grid_constant__ HwyNetParams P, const HwyNetGraph* __restrict__ graph,
+                           const __grid_constant__ HwyMergeSpawn SP, const __grid_constant__ HwyNetState S,
+                           uint64_t* __restrict__ rng, const uint8_t* __restrict__ mask_a,
+                           const uint8_t* __restrict__ mask_b) {
+    const int e = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+    const int wl = threadIdx.x & 31;
+    if (e >= S.n_envs || !env_selected(mask_a, mask_b, e)) return;  // warp-uniform
+    Pcg64 g = load_rng(rng, (size_t)S.n_envs, e);
+    const size_t base = (size_t)e * S.vp;
+    const int lanes = SP.lanes_count;
+    int placed_lane[HWY_NET_GROUP_LARGE];  // spawned_positions as (lane id, longitudinal) pairs
+    double placed_lon[HWY_NET_GROUP_LARGE];
+    int n = 0, n_placed = 0;
+    // Vehicle(road, position, heading 0, speed) into slot n: its closest lane at heading 0 (objects.py:46-50); DELTA 4,
+    // as randomize_behavior is not called, and no route
+    auto place = [&](double px, double py, double speed, double target_speed, int kind) {
+        const int lane = warp_closest_lane(graph, px, py, 0.0, wl);
+        if (wl == 0) {
+            store_vehicle(P, S, base + n, px, py, 0.0, speed, target_speed, 4.0, lane, lane, kind);
+            S.route_len[base + n] = 0;
+        }
+        ++n;
+    };
+    double px, py;
+    {  // :328-336 the ego on ("a","b",lanes-1) at s = 30, speed 30; 30 is recorded on lane id lanes-1
+        lane_position(graph->lanes[SP.lane_ab[0] + lanes - 1], 30.0, 0.0, px, py);
+        place(px, py, 30.0, P.target_speeds[SP.ego_speed_index], HWY_KIND_MDP);
+        placed_lane[0] = lanes - 1;
+        placed_lon[0] = 30.0;
+        n_placed = 1;
     }
+    for (int v = 0; v < SP.vehicles_count; ++v) {
+        for (int t = 0; t < 10; ++t) {
+            const int k = g.choice(lanes);  // integers(lanes): no draw for one lane
+            const double lon = g.uniform(0.0, SP.max_position);
+            bool safe = true;  // all(abs(longitudinal - p) > 15 for p on lane id k): exactly 15 rejects
+            for (int j = 0; j < n_placed; ++j)
+                if (placed_lane[j] == k && !(fabs(lon - placed_lon[j]) > 15.0)) {
+                    safe = false;
+                    break;
+                }
+            if (!safe) continue;
+            lane_position(graph->lanes[SP.lane_ab[0] + k], lon, 0.0, px, py);
+            const double speed = 30.0 + g.uniform(-2.0, 2.0);
+            place(px, py, speed, speed, HWY_KIND_IDM);
+            placed_lane[n_placed] = k;
+            placed_lon[n_placed] = lon;
+            ++n_placed;
+            break;
+        }
+    }
+    // :363-368 the merging vehicle on ("j","k",0) at s = 30 + 30, speed 20, target speed 30
+    lane_position(graph->lanes[SP.lane_jk], 60.0, 0.0, px, py);
+    place(px, py, 20.0, 30.0, HWY_KIND_IDM);
+    place(SP.obstacle_x, SP.obstacle_y, 0.0, 0.0, HWY_KIND_OBSTACLE);  // road.objects come after road.vehicles
+    clear_slots_past(S, base, n, wl);
     if (wl == 0) store_env_tail(S, rng, e, SP.ego_speed_index, n, g);
 }
 
@@ -2560,6 +2623,7 @@ int validate_net(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetSt
     if (s->vp != HWY_NET_GROUP && s->vp != HWY_NET_GROUP_LARGE) return fail("%s", "slot stride must be 8 or 32");
     if (p->n_vehicles < 1 || p->n_vehicles > s->vp) return fail("%s", "n_vehicles out of range for the network kernels");
     if (p->n_target_speeds < 1 || p->n_target_speeds > 3) return fail("%s", "network kernels support up to 3 target speeds");
+    if (p->merge_end_lane < 0 || p->merge_end_lane >= HWY_NET_MAX_LANES) return fail("%s", "merge_end_lane out of range");
     if (p->obs_type != HWY_OBS_KINEMATICS && p->obs_type != HWY_OBS_TTC && p->obs_type != HWY_OBS_OCCUPANCY)
         return fail("%s", "unknown obs_type");
     if (p->obs_type == HWY_OBS_TTC && (p->ttc_horizon * p->policy_frequency < 1 || p->ttc_horizon * p->policy_frequency > 16))
@@ -2878,10 +2942,24 @@ int hwy_network_reset(const HwyNetParams* p, const HwyNetGraph* graph, const Hwy
         return scripted_reset(hwynet::roundabout_generic_reset_kernel, "roundabout_generic_reset_kernel", 32,
                               p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
     }
-    case HWY_SCENARIO_MERGE:
-        if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "merge-v0: 5 vehicles + 1 obstacle on 8 slots");
-        return scripted_reset(hwynet::merge_reset_kernel, "merge_reset_kernel", 1,
-                              p, graph, sc->u.merge, s, mask_a, mask_b, obs, final_obs, st);
+    case HWY_SCENARIO_MERGE: {
+        const HwyMergeSpawn& sp = sc->u.merge;
+        if (sp.lanes_count == 0) {
+            if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "merge-v0: 5 vehicles + 1 obstacle on 8 slots");
+            return scripted_reset(hwynet::merge_reset_kernel, "merge_reset_kernel", 1,
+                                  p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+        }
+        // merge-generic: the ego, vehicles_count traffic vehicles, the merging vehicle and the Obstacle
+        if (!s->count) return fail("%s", "merge-generic: the count buffer receives the population");
+        if (sp.lanes_count < 1 || sp.lanes_count > 9) return fail("%s", "merge-generic: lanes_count out of 1..9");
+        if (sp.vehicles_count > s->vp - 3 || p->n_vehicles < 3 + (sp.vehicles_count > 0 ? sp.vehicles_count : 0))
+            return fail("%s", "merge-generic: vehicles_count exceeds the slots or n_vehicles");
+        if (sp.lane_ab[0] < 0 || sp.lane_ab[0] + sp.lanes_count > HWY_NET_MAX_LANES || sp.lane_jk < 0 ||
+            sp.lane_jk >= HWY_NET_MAX_LANES)
+            return fail("%s", "merge-generic: lane index out of range");
+        return scripted_reset(hwynet::merge_generic_reset_kernel, "merge_generic_reset_kernel", 32,  // a warp per env
+                              p, graph, sp, s, mask_a, mask_b, obs, final_obs, st);
+    }
     case HWY_SCENARIO_TWO_WAY:
         if (s->vp != HWY_NET_GROUP || p->n_vehicles != 6) return fail("%s", "two-way-v0: 6 vehicles on 8 slots");
         return scripted_reset(hwynet::two_way_reset_kernel, "two_way_reset_kernel", 1,

@@ -27,6 +27,7 @@ from .. import _native as N
 from ..road.network import NetworkTable
 from ..spaces import Discrete, batch_space
 from .common.action import DiscreteMetaAction, speed_to_index
+from .common.config_road import ConfigRoadMixin
 from .common.observation import select_network_observation
 from .common.vector_env import BatchedNetworkEnv
 
@@ -381,7 +382,7 @@ def check_roundabout_generic(cfg: dict, env_id: str) -> None:
         raise IndexError("list index out of range")  # destinations[min(d, 3)] in the reference
 
 
-class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
+class BatchedRoundaboutGenericEnv(ConfigRoadMixin, BatchedRoundaboutEnv):
     """`roundabout-generic-v0`: RoundaboutGenericEnv (roundabout_env.py:398-751), RoundaboutEnv's rewards, termination
     and dynamics on a roundabout of config["roundabout_lanes"] ring lanes (1..2) at config["roundabout_radius"], with
     config["vehicles_count"] traffic vehicles placed by rejection sampling (HWY_SCENARIO_ROUNDABOUT_GENERIC).  A
@@ -390,30 +391,16 @@ class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
     The lane table follows the config: reset(options={"config": ...}) rebuilds it and re-allocates."""
 
     ENV_ID = "roundabout-generic-v0"
-
-    def _make_network(self) -> NetworkTable:
-        return self._road
+    ROAD_KEYS = ("roundabout_radius", "roundabout_lanes")
 
     def define_spaces(self) -> None:
         if self.reset_mode != "device":
             raise NotImplementedError(f"{self.ENV_ID} resets on the device")
         cfg = self.config
         check_roundabout_generic(cfg, self.ENV_ID)
-        road = roundabout_generic_network(cfg["roundabout_radius"], cfg["roundabout_lanes"])
-        if self._net is not road:  # another (radius, lanes): rebuild the device table
-            self._net = None
-        self._road = road
-        count = int(cfg["vehicles_count"])
-        self.N_VEHICLES = 1 + max(count, 0)
-        self.SLOTS = N.HWY_NET_GROUP if self.N_VEHICLES <= N.HWY_NET_GROUP else N.HWY_NET_GROUP_LARGE
+        self._use_road(roundabout_generic_network(cfg["roundabout_radius"], cfg["roundabout_lanes"]),
+                       1 + max(int(cfg["vehicles_count"]), 0))
         super().define_spaces()
-
-    def _allocate(self) -> None:
-        super()._allocate()  # the 32-slot state already carries the population and the (unused) rule clock
-        if self.vp == N.HWY_NET_GROUP:  # the 8-slot kernels read the population when the state carries one
-            self._count = torch.full((self.num_envs,), self.N_VEHICLES, dtype=torch.int32, device=self.device)
-            self._state.count = self._count.data_ptr()
-            self._road_steps = None
 
     def _build_spawn_tables(self) -> None:
         net, cfg = self.net, self.config
@@ -430,31 +417,6 @@ class BatchedRoundaboutGenericEnv(BatchedRoundaboutEnv):
         s.route_table, s.route_len = self._route_table.data_ptr(), self._route_table_len.data_ptr()
         self._scenario = N.HwyNetScenario(kind=N.HWY_SCENARIO_ROUNDABOUT_GENERIC,
                                           u=N.HwyNetScenarioUnion(roundabout_generic=s))
-
-    def to_finite_mdp(self):
-        raise NotImplementedError(f"to_finite_mdp on {self.ENV_ID}")
-
-    def copy_envs(self, dst_ids, src_ids, source=None) -> None:
-        """BatchedVectorEnv.copy_envs; two envs of one class may still run different lane tables (radius, lanes) or
-        slot strides, and a state only means something on its own table."""
-        if source is not None and type(source) is type(self) and (source._road is not self._road
-                                                                   or source.vp != self.vp):
-            raise ValueError(f"copy_envs between {self.ENV_ID} envs on different roads (roundabout_radius, "
-                             "roundabout_lanes) or slot strides")
-        super().copy_envs(dst_ids, src_ids, source)
-
-    def state_dict(self) -> dict:
-        """RoundaboutEnv's fields [N, V] with V = 1 + vehicles_count; `count` vehicles of each env are on the road."""
-        sd = super().state_dict()
-        sd["count"] = self._count.cpu().numpy()
-        return sd
-
-    def load_state_dict(self, sd: dict, env_ids=None) -> None:
-        super().load_state_dict(sd, env_ids)
-        idx = slice(None) if env_ids is None else torch.from_numpy(np.asarray(env_ids, dtype=np.int64)).to(self.device)
-        self._count[idx] = torch.from_numpy(np.asarray(sd["count"], dtype=np.int32).reshape(-1)).to(self.device)
-        if self._road_steps is not None:
-            self._road_steps[idx] = 0
 
 
 class BatchedConnectedLaneRoundaboutGenericEnv(BatchedRoundaboutGenericEnv):

@@ -298,8 +298,9 @@ typedef struct HwyNetParams {
     double arrived_reward, reward_speed_lo, reward_speed_hi;
     /* merge-v0 (envs/merge_env.py:24-84): reward_type 2 */
     double right_lane_reward, merging_speed_reward;
-    int32_t merge_lane;         /* table index of ("b", "c", 2): slow ControlledVehicles there are penalised */
-    int32_t _pad_merge;
+    int32_t merge_lane;         /* table index of ("b", "c", 2): slow ControlledVehicles there are penalised; -1: none */
+    int32_t merge_end_lane;     /* 0: terminated past x = 370 (merge-v0); > 0: table index of a ("c","d",k) lane,
+                                 * terminated past its end x - 90 (MergeGenericEnv.end_position, merge_env.py:249) */
     double left_lane_reward;    /* two-way-v0 (envs/two_way_env.py:17-62): reward_type 3; u-turn-v0
                                  * (envs/u_turn_env.py:14-82): reward_type 4 */
     /* exit-v0 (envs/exit_env.py:147-198): reward_type 5 = collision, goal (the TARGET lane is ("1","2",lanes_count) or
@@ -454,6 +455,20 @@ typedef struct HwyMergeSpawn {
     int32_t lane_jk;         /* ("j","k",0) */
     int32_t ego_speed_index; /* MDPVehicle.speed_to_index(30) */
     double obstacle_x, obstacle_y;
+    /* merge-generic-v0 / v1 (MergeGenericEnv._make_vehicles, envs/merge_env.py:320-368) when lanes_count > 0: the
+     * MDPVehicle on ("a","b",lanes_count-1) at s = 30, speed 30; then for each of vehicles_count vehicles up to 10
+     * tries of integers(lanes_count) (no draw for one lane) and uniform(0, max_position), rejected unless the
+     * longitudinal lies more than 15 m from every one already placed on that lane id (the ego's 30 included); an
+     * accepted try draws its speed 30 + uniform(-2, 2) and is placed at ("a","b",k).position(s, 0), which may lie past
+     * the lane's end.  Then the merging IDM vehicle on ("j","k",0) at s = 60, speed 20, target speed 30, and the
+     * Obstacle last.  Every object takes its closest lane at heading 0.  Lane k of ("a","b") is lane_ab[0] + k.  A
+     * vehicle whose 10 tries fail is skipped: s->count (required) receives the population (the Obstacle's slot is
+     * count - 1) and the slots past it are cleared.  Slot stride 8 or 32; on 32 slots the step is the one without
+     * rules or population changes.  This tail grew the struct from 32 to 48 bytes inside the union, whose size and
+     * offset did not change (the union's largest member is HwyUTurnSpawn). */
+    int32_t lanes_count;     /* config["lanes_count"], 1..9; 0: merge-v0's fixed placement above */
+    int32_t vehicles_count;  /* config["vehicles_count"], at most s->vp - 3 (<= 0: no traffic) */
+    double max_position;     /* before + converge + parallel merge lengths, the traffic's uniform upper bound */
 } HwyMergeSpawn;
 
 /* u-turn-v0 (HWY_SCENARIO_U_TURN): UTurnEnv._make_vehicles (envs/u_turn_env.py:179-275) on the device: the
