@@ -94,6 +94,7 @@ struct EnvShared {
     uint32_t ctrl[NW], cc[NW];               // ControlledVehicle instances / check_collisions
     int last_will[TPE];                      // collision sweep: largest partner with will_intersect
     unsigned char crash_hit[TPE];
+    double2 will_imp[TPE];                   // single checker: (trx, try) of the pair (0, j), written by vehicle j
     // fused autoreset staging (Vehicle.create_random chain): per-vehicle spawn increment / position
     double sp_x[TPE];
     int done, sp_fallback;
@@ -847,9 +848,11 @@ __device__ __noinline__ void warp_order(Frame<TPE>& F, const Frame<TPE>& prev, i
 // After a barrier that follows publish(): ranks, rank-ordered membership masks, lane / target
 // masks (warp ballots) and the first pass of the collision sweep of Road.step
 // (road/road.py:477-481).  All threads of the env call this convergently.
+// Returns true when vehicle 0 is the env's only checking vehicle (uniform over the env): then every vehicle but 0
+// has resolved its own side of the sweep in `r` here, and only vehicle 0 runs apply_collisions.
 template <int TPE, bool DENSE>
-__device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared<TPE>& sm, Frame<TPE>& F,
-                                            int i, bool active, bool aligned, const VehicleRegs& r,
+__device__ __forceinline__ bool build_frame(const HwyHighwayParams& P, EnvShared<TPE>& sm, Frame<TPE>& F,
+                                            int i, bool active, bool aligned, VehicleRegs& r,
                                             double dt, bool do_sweep, bool do_masks, bool pruned,
                                             const Frame<TPE>& prev) {
     const int V = P.n_vehicles;
@@ -974,6 +977,18 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
     // -- collision sweep, pass 1: every gated pair once.  A pair with exactly one
     // check_collisions side is taken by the other side's thread (so the controlled vehicle's
     // pairs are spread over the block); pairs of two checking vehicles are dealt round-robin.
+    // A single checking vehicle 0 (highway-fast, `single`): vehicle i > 0 takes the pair (0, i), the only one it is
+    // part of, and applies its own side at once — the crashed flag, and the impact -(trx, try) / 2 (i is the pair's
+    // second member).  Vehicle 0's side is an OR over its pairs and the impact of the largest partner with
+    // will_intersect (the last writer of the reference's (i < j) loop): a shared flag, an atomicMax, and each such
+    // pair's (trx, try) in will_imp[i], which apply_collisions reads instead of running pair_sat again.
+    bool single = false;
+    if (!pruned) {
+        uint32_t rest = 0;
+#pragma unroll
+        for (int w = 1; w < TPE / 32; ++w) rest |= sm.cc[w];
+        single = sm.cc[0] == 1u && rest == 0u;
+    }
     if (do_sweep && pruned) {
         // many checking vehicles (highway-v0: all of them): the sweep runs after the next barrier over the
         // rank-neighbours only (sweep_pruned); here just the env's speed bound.  Non-negative floats order
@@ -997,6 +1012,20 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
             bool inter, will;
             double trx, try_;
             pair_sat(F, a, b, dt, inter, will, trx, try_);
+            if (single) {  // a = 0, b = i
+                if (will) {
+                    sm.will_imp[b] = make_double2(trx, try_);
+                    atomicMax(&sm.last_will[a], b);
+                    r.imp_x = -trx / 2;
+                    r.imp_y = -try_ / 2;
+                    r.meta |= HWY_META_HAS_IMPACT;
+                }
+                if (inter) {
+                    sm.crash_hit[a] = 1;
+                    r.meta |= HWY_META_CRASHED;
+                }
+                return;
+            }
             if (will) {
                 atomicMax(&sm.last_will[a], b);
                 atomicMax(&sm.last_will[b], a);
@@ -1022,6 +1051,7 @@ __device__ __forceinline__ void build_frame(const HwyHighwayParams& P, EnvShared
             }
         }
     }
+    return single;
 }
 
 // Collision sweep, pass 1, rank-pruned form (after the barrier that follows build_frame).  The frame holds every
@@ -1058,10 +1088,10 @@ __device__ __forceinline__ void sweep_pruned(EnvShared<TPE>& sm, const Frame<TPE
 // Collision sweep, pass 2 (own slot): `crashed` is an OR over the intersecting partners, the
 // impact is the one of the LAST writer in the reference's (i < j) double loop = the largest
 // partner index with will_intersect (vehicle/objects.py:103-116).  SAT is recomputed for that
-// one pair (deterministic, rare).
+// one pair (deterministic, rare), except with a single checking vehicle (`single`, i = 0), whose partner left it.
 template <int TPE>
 __device__ __forceinline__ void apply_collisions(EnvShared<TPE>& sm, const Frame<TPE>& F, int i,
-                                                 VehicleRegs& r, double dt) {
+                                                 VehicleRegs& r, double dt, bool single) {
     if (sm.crash_hit[i]) {
         r.meta |= HWY_META_CRASHED;
         sm.crash_hit[i] = 0;
@@ -1071,7 +1101,12 @@ __device__ __forceinline__ void apply_collisions(EnvShared<TPE>& sm, const Frame
         int a = i < j ? i : j, b = i < j ? j : i;
         bool inter, will;
         double trx, try_;
-        pair_sat(F, a, b, dt, inter, will, trx, try_);
+        if (single) {
+            trx = sm.will_imp[j].x;
+            try_ = sm.will_imp[j].y;
+        } else {
+            pair_sat(F, a, b, dt, inter, will, trx, try_);
+        }
         r.imp_x = i == a ? trx / 2 : -trx / 2;
         r.imp_y = i == a ? try_ / 2 : -try_ / 2;
         r.meta |= HWY_META_HAS_IMPACT;

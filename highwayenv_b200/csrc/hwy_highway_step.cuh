@@ -117,7 +117,8 @@
         // frame 0: masks only — the sweep of the stored state ran at the end of the substep that
         // produced it (previous launch).  Later: Road.step's sweep (road/road.py:477-481).  The last frame: ranks and
         // the sweep, no masks.
-        build_frame<TPE, DENSE>(P, sm, F, i, active, aligned, r, dt, frame > 0, acts, pruned, sm.f[p ^ 1]);
+        const bool single =
+            build_frame<TPE, DENSE>(P, sm, F, i, active, aligned, r, dt, frame > 0, acts, pruned, sm.f[p ^ 1]);
         PHASE_MARK(3);  // ranks, masks, sweep pass 1
         if (pruned && frame > 0) {  // uniform over the grid
             env_sync_phase<TPE, 3>();
@@ -125,7 +126,7 @@
         }
         env_sync_phase<TPE, 3>();
         PHASE_MARK(4);  // barrier after build
-        if (active && frame > 0) apply_collisions(sm, F, i, r, dt);
+        if (active && frame > 0 && (!single || i == 0)) apply_collisions(sm, F, i, r, dt, single);
         PHASE_MARK(5);  // sweep pass 2
         if (frame == frames) break;
 
