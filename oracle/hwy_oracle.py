@@ -99,6 +99,11 @@ _F64 = ("x", "y", "heading", "speed", "target_speed", "timer", "delta", "impact_
 _I32 = ("lane", "target_lane", "kind", "crashed", "has_impact", "check_collisions")
 
 
+class OrcHighwayState(C.Structure):
+    _fields_ = [(k, C.c_void_p) for k in _F64] + [(k, C.c_void_p) for k in _I32] + [
+        ("speed_index", C.c_void_p), ("time", C.c_void_p)]
+
+
 class OrcBatch(C.Structure):
     _fields_ = (
         [("n_envs", C.c_int32)]
@@ -152,6 +157,10 @@ def lib():
         _lib.orc_highway_reset_batch.argtypes = [
             C.POINTER(OrcHighwayCfg), C.POINTER(OrcBatch), C.c_void_p, C.c_void_p, C.c_int,
         ]
+        _lib.orc_highway_substeps.restype = None
+        _lib.orc_highway_substeps.argtypes = [C.POINTER(OrcHighwayCfg), C.POINTER(OrcHighwayState), C.c_int]
+        _lib.orc_highway_observe.restype = None
+        _lib.orc_highway_observe.argtypes = [C.POINTER(OrcHighwayCfg), C.POINTER(OrcHighwayState), C.c_void_p]
         _lib.orc_highway_step_batch.restype = None
         _lib.orc_highway_step_batch.argtypes = [
             C.POINTER(OrcHighwayCfg), C.POINTER(OrcBatch), C.c_void_p, C.c_void_p, C.c_void_p,
@@ -297,6 +306,25 @@ class OracleBatch:
             self.truncated.ctypes.data, int(autoreset), self.threads,
         )
         return self.obs, self.reward, self.terminated, self.truncated
+
+    def env_state(self, e: int) -> OrcHighwayState:
+        """env slot e as the single-env OrcHighwayState of orc_highway_substeps / orc_highway_observe (views of the
+        batch arrays)"""
+        st = OrcHighwayState()
+        for k in list(_F64) + list(_I32):
+            setattr(st, k, self.a[k][e].ctypes.data)
+        st.speed_index = self.a["speed_index"][e:].ctypes.data
+        st.time = self.a["time"][e:].ctypes.data
+        return st
+
+    def substeps(self, e: int, n: int) -> None:
+        """n x (Road.act(); Road.step(dt)) on env slot e"""
+        lib().orc_highway_substeps(C.byref(self.cfg), C.byref(self.env_state(e)), int(n))
+
+    def observe(self, e: int) -> np.ndarray:
+        out = np.zeros(self.obs.shape[1:], dtype=np.float32)
+        lib().orc_highway_observe(C.byref(self.cfg), C.byref(self.env_state(e)), out.ctypes.data)
+        return out
 
     def load_state(self, e: int, st: dict):
         """Inject a state dumped by ref_harness.dump_state into env slot e."""
