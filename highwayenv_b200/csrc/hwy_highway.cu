@@ -23,13 +23,16 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
-#include <atomic>
 #include <cstddef>
+#include <map>
 #include <mutex>
+#include <type_traits>
+#include <utility>
 
 #include <cuda_runtime.h>
 
 #include "../../include/hwyb200.h"
+#include "hwy_abi.h"
 #include "hwy_device.cuh"
 #include "hwy_math.cuh"
 
@@ -1440,15 +1443,9 @@ __device__ __forceinline__ void spawn_fused(const HwyHighwayParams& P, const Hwy
 }
 
 // ------------------------------------------------------------------ the step kernel
-constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full register file
-// Register budget of the step kernel = 65536 / (HWY_STEP_BOUND_THREADS * HWY_STEP_BOUND_BLOCKS); the launcher never
-// uses more than HWY_STEP_BOUND_THREADS threads per block.  (512, 1): 128 registers, two 256-thread blocks per SM.
-#ifndef HWY_STEP_BOUND_THREADS
-#define HWY_STEP_BOUND_THREADS 512
-#endif
-#ifndef HWY_STEP_BOUND_BLOCKS
-#define HWY_STEP_BOUND_BLOCKS 1
-#endif
+// Register budget of the step kernel = 65536 / kMaxBlockThreads: 128 registers, two 256-thread blocks per SM.  The
+// launcher never uses more than kMaxBlockThreads threads per block.
+constexpr int kMaxBlockThreads = 512;
 
 // blockDim.x = TPE * (envs per block); dynamic shared memory = envs per block * sizeof(EnvShared).
 // DENSE (see launch_step): `dense_epb` envs per block, env `sub` on the V threads from sub * V, vehicle
@@ -1465,7 +1462,7 @@ constexpr int kMaxBlockThreads = 512;  // 128 registers/thread => one full regis
 // staging follows its EnvShared array in dynamic shared memory).  Only `if constexpr (LINEAR)` branches differ, and
 // each kernel keeps the body in its own scope (an inlined device function changes the IDM kernel's code schedule).
 template <int TPE, bool AL, bool DENSE>
-__global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
+__global__ void __launch_bounds__(kMaxBlockThreads, 1)
 highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                     const int32_t* __restrict__ action_i, const float* __restrict__ action_f,
                     float* __restrict__ obs, double* __restrict__ reward,
@@ -1479,7 +1476,7 @@ highway_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighway
 
 // LinearVehicle / AggressiveVehicle / DefensiveVehicle traffic (vehicle/behavior.py:350-583)
 template <int TPE, bool AL, bool DENSE>
-__global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
+__global__ void __launch_bounds__(kMaxBlockThreads, 1)
 highway_linear_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                            const __grid_constant__ HwyLinearTraffic T_, const int32_t* __restrict__ action_i,
                            const float* __restrict__ action_f, float* __restrict__ obs, double* __restrict__ reward,
@@ -1634,7 +1631,7 @@ __global__ void debug_pcg64_kernel(int op, int arg_i, double arg_lo, double arg_
 // autoreset spawns the multi-agent layout (spawn_bin).  Lane tables are always congruent (AL) on this path.  The
 // block's MultiShared staging follows its EnvShared array in dynamic shared memory.
 template <int TPE, bool DENSE>
-__global__ void __launch_bounds__(HWY_STEP_BOUND_THREADS, HWY_STEP_BOUND_BLOCKS)
+__global__ void __launch_bounds__(kMaxBlockThreads, 1)
 highway_multi_step_kernel(const __grid_constant__ HwyHighwayParams P, const HwyHighwayState S,
                           const int32_t* __restrict__ action_i, const float* __restrict__ action_f,
                           float* __restrict__ obs, double* __restrict__ reward,
@@ -1713,6 +1710,50 @@ int check_launch(const char* what) {
     }
     return 0;
 }
+int require_device() {
+    int dev_count = 0;
+    if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count < 1) {
+        cudaGetLastError();
+        return fail("%s", "no CUDA device: this library has no CPU fallback");
+    }
+    return 0;
+}
+int current_device(int& dev) {
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
+    return 0;
+}
+int device_props(DeviceProps& out) {
+    static std::mutex mu;
+    static DeviceProps props[64];
+    static bool ready[64] = {false};
+    int dev = 0;
+    if (current_device(dev)) return 1;
+    std::lock_guard<std::mutex> lock(mu);
+    if (!ready[dev]) {
+        DeviceProps& d = props[dev];
+        cudaError_t err = cudaDeviceGetAttribute(&d.n_sm, cudaDevAttrMultiProcessorCount, dev);
+        if (err == cudaSuccess) err = cudaDeviceGetAttribute(&d.smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+        if (err == cudaSuccess) err = cudaDeviceGetAttribute(&d.smem_block, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        if (err != cudaSuccess) return fail("cudaDeviceGetAttribute: %s", cudaGetErrorString(err));
+        ready[dev] = true;
+    }
+    out = props[dev];
+    return 0;
+}
+// The attribute is per kernel and device; the lock makes the check and the raise one step.
+int opt_in_smem(const void* kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, size_t> raised;
+    int dev = 0;
+    if (current_device(dev)) return 1;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& limit = raised[{kernel, dev}];
+    if (bytes <= limit) return 0;
+    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
+    limit = bytes;
+    return 0;
+}
 }  // namespace hwy_abi
 
 namespace {
@@ -1743,14 +1784,16 @@ int validate(const HwyHighwayParams* p, const HwyHighwayState* s) {
     if (!s->pos || !s->hs || !s->tt || !s->imp || !s->delta || !s->meta || !s->speed_index ||
         !s->time || !s->rng)
         return fail("%s", "null state pointer");
-    int dev_count = 0;
-    if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count < 1) {
-        cudaGetLastError();
-        return fail("%s", "no CUDA device: this library has no CPU fallback");
-    }
-    return 0;
+    return hwy_abi::require_device();
 }
-int tpe_for(int n_vehicles) { return n_vehicles <= 32 ? 32 : (n_vehicles <= 64 ? 64 : 128); }
+// f(std::integral_constant<int, TPE>{}) for the n_vehicles-thread env segments: TPE = 32, 64 or 128, the next power of
+// two >= n_vehicles, sizes the step and observe kernels' per-env shared arrays
+template <typename F>
+int with_tpe(int n_vehicles, F f) {
+    if (n_vehicles <= 32) return f(std::integral_constant<int, 32>{});
+    if (n_vehicles <= 64) return f(std::integral_constant<int, 64>{});
+    return f(std::integral_constant<int, 128>{});
+}
 
 struct Grid {
     int blocks, threads;
@@ -1760,37 +1803,12 @@ Grid grid_for(int tpe, int n_envs) {
     return Grid{(n_envs + epb - 1) / epb, tpe * epb};
 }
 
-int step_block_thread_limit() {
-    return hwy::kMaxBlockThreads < HWY_STEP_BOUND_THREADS ? hwy::kMaxBlockThreads : HWY_STEP_BOUND_THREADS;
-}
-int step_half_block_threads() { return step_block_thread_limit() / 2; }
 // Envs per block of the step kernel: as many V-thread envs as fit half the block-thread limit (two blocks per SM),
 // reduced when that leaves the last wave of blocks mostly empty.  HWYB200_EPB overrides, up to the whole limit.  Both
 // are also bounded by shared memory (env_bytes per env), which only binds below V = 17.
-struct StepDevice {
-    int n_sm, smem_sm, smem_block;  // SMs, shared memory per SM, opt-in shared memory per block
-};
-// read once per device
-const StepDevice& step_device(int dev) {
-    static StepDevice info[64];
-    static std::atomic<bool> ready[64];
-    static std::mutex mu;
-    if (!ready[dev].load(std::memory_order_acquire)) {
-        std::lock_guard<std::mutex> lock(mu);
-        if (!ready[dev].load(std::memory_order_relaxed)) {
-            StepDevice d{132, 228 * 1024, 227 * 1024};
-            cudaDeviceGetAttribute(&d.n_sm, cudaDevAttrMultiProcessorCount, dev);
-            cudaDeviceGetAttribute(&d.smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
-            cudaDeviceGetAttribute(&d.smem_block, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-            info[dev] = d;
-            ready[dev].store(true, std::memory_order_release);
-        }
-    }
-    return info[dev];
-}
-int step_envs_per_block(int n_vehicles, size_t env_bytes, int n_envs, const StepDevice& d) {
-    const int limit = step_block_thread_limit();
-    int max_epb = std::min<long>(limit / n_vehicles, d.smem_block / (long)env_bytes);
+constexpr int kHalfBlockThreads = hwy::kMaxBlockThreads / 2;
+int step_envs_per_block(int n_vehicles, size_t env_bytes, int n_envs, const hwy_abi::DeviceProps& d) {
+    int max_epb = std::min<long>(hwy::kMaxBlockThreads / n_vehicles, d.smem_block / (long)env_bytes);
     if (max_epb < 1) max_epb = 1;
     if (const char* e = getenv("HWYB200_EPB")) {
         int v = atoi(e);
@@ -1798,7 +1816,7 @@ int step_envs_per_block(int n_vehicles, size_t env_bytes, int n_envs, const Step
     }
     // Two resident blocks per SM (rather than one block of max_epb envs or many 1-env blocks): the blocks cover each other's
     // barrier stalls.  Small batches shrink the block so every SM still gets work.
-    int epb = std::min<long>(step_half_block_threads() / n_vehicles, (d.smem_sm / 2 - 1024) / (long)env_bytes);
+    int epb = std::min<long>(kHalfBlockThreads / n_vehicles, (d.smem_sm / 2 - 1024) / (long)env_bytes);
     if (epb < 1) epb = 1;
     while (epb > 1 && (long)n_envs < (long)epb * 2 * d.n_sm) --epb;
     return epb;
@@ -1812,7 +1830,7 @@ int ensure_pcg_jump(cudaStream_t st) {
     static std::mutex mu;
     static bool ready[64] = {false};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
+    if (hwy_abi::current_device(dev)) return 1;
     std::lock_guard<std::mutex> lock(mu);
     if (ready[dev]) return 0;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -1848,77 +1866,41 @@ bool lanes_congruent_host(const HwyHighwayParams* p) {
     return ok;
 }
 
-template <int TPE, bool AL, bool DENSE>
-int launch_step_kernel(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                       const int32_t* action_i, const float* action_f, float* obs, double* reward,
-                       uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
-                       int autoreset, float* final_obs, int epb, size_t env_bytes, int dev, cudaStream_t st) {
-    const int blocks = (s->n_envs + epb - 1) / epb;
-    const size_t smem = (size_t)epb * env_bytes;
-    // the attribute is per device (and per template instance): cache it by device ordinal
-    static std::atomic<size_t> configured[2][64];
-    if (smem > configured[t != nullptr][dev].load(std::memory_order_relaxed)) {
-        cudaError_t err = t ? cudaFuncSetAttribute(hwy::highway_linear_step_kernel<TPE, AL, DENSE>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                            : cudaFuncSetAttribute(hwy::highway_step_kernel<TPE, AL, DENSE>,
-                                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-        configured[t != nullptr][dev].store(smem, std::memory_order_relaxed);
-    }
-    const int threads = DENSE ? (epb * p->n_vehicles + 31) & ~31 : epb * TPE;
-    if (t)
-        hwy::highway_linear_step_kernel<TPE, AL, DENSE><<<blocks, threads, smem, st>>>(
-            *p, *s, *t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-            autoreset, final_obs, epb);
-    else
-        hwy::highway_step_kernel<TPE, AL, DENSE><<<blocks, threads, smem, st>>>(
-            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed,
-            autoreset, final_obs, epb);
-    return 0;
-}
-
-// t == nullptr: IDMVehicle traffic (highway_step_kernel); else LinearVehicle traffic (highway_linear_step_kernel)
-template <int TPE, bool AL>
-int launch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
-                const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
-                uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset,
-                float* final_obs, cudaStream_t st) {
+// One launch of a step kernel.  dense / sparse: its DENSE = true / false instantiations; extra_bytes: the per-env
+// staging that follows the block's EnvShared array in dynamic shared memory (LinearShared, MultiShared or none); args:
+// the kernel's parameters before dense_epb.
+template <int TPE, typename... Params, typename... Args>
+int launch_step(void (*dense)(Params...), void (*sparse)(Params...), size_t extra_bytes, const char* name,
+                const HwyHighwayParams* p, const HwyHighwayState* s, int autoreset, cudaStream_t st,
+                const Args&... args) {
     if (autoreset > 0 && ensure_pcg_jump(st)) return 1;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
-    const size_t env_bytes = sizeof(hwy::EnvShared<TPE>) + (t ? sizeof(hwy::LinearShared<TPE>) : 0);
-    const int epb = step_envs_per_block(p->n_vehicles, env_bytes, s->n_envs, step_device(dev));
+    hwy_abi::DeviceProps d;
+    if (hwy_abi::device_props(d)) return 1;
+    const size_t env_bytes = sizeof(hwy::EnvShared<TPE>) + extra_bytes;
+    const int epb = step_envs_per_block(p->n_vehicles, env_bytes, s->n_envs, d);
     // Dense segments (V threads per env, the DENSE kernels) only where they put more envs into a block than TPE-thread
     // segments; otherwise the TPE-thread kernel runs, which carries none of the segment bookkeeping.
-    const bool dense = epb * TPE > step_half_block_threads();
-    if (dense)
-        return launch_step_kernel<TPE, AL, true>(p, s, t, action_i, action_f, obs, reward, terminated, truncated,
-                                                 info_speed, info_crashed, autoreset, final_obs, epb, env_bytes, dev,
-                                                 st);
-    return launch_step_kernel<TPE, AL, false>(p, s, t, action_i, action_f, obs, reward, terminated, truncated,
-                                              info_speed, info_crashed, autoreset, final_obs, epb, env_bytes, dev, st);
+    const bool is_dense = epb * TPE > kHalfBlockThreads;
+    const auto kernel = is_dense ? dense : sparse;
+    const size_t smem = (size_t)epb * env_bytes;
+    if (hwy_abi::opt_in_smem((const void*)kernel, smem)) return 1;
+    const int threads = is_dense ? (epb * p->n_vehicles + 31) & ~31 : epb * TPE;
+    kernel<<<(s->n_envs + epb - 1) / epb, threads, smem, st>>>(args..., epb);
+    return check_launch(name);
 }
 
 int launch_observe(const HwyHighwayParams* p, const HwyHighwayState* s, const uint8_t* mask_a,
                    const uint8_t* mask_b, float* obs, cudaStream_t st) {
-    int tpe = tpe_for(p->n_vehicles);
-    Grid g = grid_for(tpe, s->n_envs);
-    if (p->n_agents > 1) {
-        if (tpe == 32)
-            hwy::highway_multi_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-        else if (tpe == 64)
-            hwy::highway_multi_observe_kernel<64><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-        else
-            hwy::highway_multi_observe_kernel<128><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-        return check_launch("highway_multi_observe_kernel");
-    }
-    if (tpe == 32)
-        hwy::highway_observe_kernel<32><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-    else if (tpe == 64)
-        hwy::highway_observe_kernel<64><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-    else
-        hwy::highway_observe_kernel<128><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
-    return check_launch("highway_observe_kernel");
+    return with_tpe(p->n_vehicles, [&](auto tpe) {
+        constexpr int TPE = decltype(tpe)::value;
+        const Grid g = grid_for(TPE, s->n_envs);
+        if (p->n_agents > 1) {
+            hwy::highway_multi_observe_kernel<TPE><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
+            return check_launch("highway_multi_observe_kernel");
+        }
+        hwy::highway_observe_kernel<TPE><<<g.blocks, g.threads, 0, st>>>(*p, *s, mask_a, mask_b, obs);
+        return check_launch("highway_observe_kernel");
+    });
 }
 
 // t == nullptr: IDMVehicle traffic (highway_reset_kernel); else LinearVehicle traffic (highway_linear_reset_kernel)
@@ -1949,86 +1931,49 @@ int check_step_args(const HwyHighwayParams* p, const HwyHighwayState* s, const i
     return 0;
 }
 
-int dispatch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                        const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
-                        double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st);
-
+// t == nullptr: IDMVehicle traffic (highway_step_kernel); else LinearVehicle traffic (highway_linear_step_kernel).
+// Several controlled vehicles (n_agents > 1): highway_multi_step_kernel, on congruent lane tables only.
+// The order in which the kernels are named here is their order in the module, and the DENSE kernels' constant-bank
+// layout follows it: the multi-agent kernels come after every single-agent one.
 int dispatch_step(const HwyHighwayParams* p, const HwyHighwayState* s, const HwyLinearTraffic* t,
                   const int32_t* action_i, const float* action_f, float* obs, double* reward, uint8_t* terminated,
                   uint8_t* truncated, double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs,
                   cudaStream_t st) {
-    int tpe = tpe_for(p->n_vehicles);
     // HWYB200_GENERAL_LANES=1 (tests): run the general-geometry instantiation on a congruent lane table too
     const char* force_general = getenv("HWYB200_GENERAL_LANES");
     const bool al = lanes_congruent_host(p) && !(force_general && force_general[0] == '1');
-    if (p->n_agents > 1) {
-        if (!al) return fail("%s", "several controlled vehicles need a congruent lane table (no general-geometry "
-                                   "multi-agent kernel)");
-        return dispatch_multi_step(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
-                                   info_crashed, autoreset, final_obs, st);
-    }
-#define HWY_LAUNCH_STEP(T, A)                                                                              \
-    launch_step<T, A>(p, s, t, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, \
-                      autoreset, final_obs, st)
-    int rc;
-    if (tpe == 32)
-        rc = al ? HWY_LAUNCH_STEP(32, true) : HWY_LAUNCH_STEP(32, false);
-    else if (tpe == 64)
-        rc = al ? HWY_LAUNCH_STEP(64, true) : HWY_LAUNCH_STEP(64, false);
-    else
-        rc = al ? HWY_LAUNCH_STEP(128, true) : HWY_LAUNCH_STEP(128, false);
-#undef HWY_LAUNCH_STEP
-    if (rc) return 1;
-    if (check_launch(t ? "highway_linear_step_kernel" : "highway_step_kernel")) return 1;
-    return 0;
-}
-// Several controlled vehicles (n_agents > 1): highway_multi_step_kernel, on congruent lane tables only.
-template <int TPE>
-int launch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                      const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
-                      double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st) {
-    if (autoreset > 0 && ensure_pcg_jump(st)) return 1;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
-    const size_t env_bytes = sizeof(hwy::EnvShared<TPE>) + sizeof(hwy::MultiShared<TPE>);
-    const int epb = step_envs_per_block(p->n_vehicles, env_bytes, s->n_envs, step_device(dev));
-    const bool dense = epb * TPE > step_half_block_threads();
-    const int blocks = (s->n_envs + epb - 1) / epb;
-    const size_t smem = (size_t)epb * env_bytes;
-    static std::atomic<size_t> configured[2][64];
-    if (smem > configured[dense][dev].load(std::memory_order_relaxed)) {
-        cudaError_t err = dense ? cudaFuncSetAttribute(hwy::highway_multi_step_kernel<TPE, true>,
-                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-                                : cudaFuncSetAttribute(hwy::highway_multi_step_kernel<TPE, false>,
-                                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-        configured[dense][dev].store(smem, std::memory_order_relaxed);
-    }
-    if (dense)
-        hwy::highway_multi_step_kernel<TPE, true><<<blocks, (epb * p->n_vehicles + 31) & ~31, smem, st>>>(
-            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, autoreset,
-            final_obs, epb);
-    else
-        hwy::highway_multi_step_kernel<TPE, false><<<blocks, epb * TPE, smem, st>>>(
-            *p, *s, action_i, action_f, obs, reward, terminated, truncated, info_speed, info_crashed, autoreset,
-            final_obs, epb);
-    return check_launch("highway_multi_step_kernel");
-}
-
-// (after dispatch_step: the multi-agent kernels are instantiated after every single-agent one, whose code and
-// constant-bank layout then stay as they were)
-int dispatch_multi_step(const HwyHighwayParams* p, const HwyHighwayState* s, const int32_t* action_i,
-                        const float* action_f, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
-                        double* info_speed, uint8_t* info_crashed, int autoreset, float* final_obs, cudaStream_t st) {
-    const int tpe = tpe_for(p->n_vehicles);
-    if (tpe == 32)
-        return launch_multi_step<32>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
-                                     info_crashed, autoreset, final_obs, st);
-    if (tpe == 64)
-        return launch_multi_step<64>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
-                                     info_crashed, autoreset, final_obs, st);
-    return launch_multi_step<128>(p, s, action_i, action_f, obs, reward, terminated, truncated, info_speed,
-                                  info_crashed, autoreset, final_obs, st);
+    // head: the kernel's parameters before the ones every step kernel shares
+    auto launch = [&](auto tpe, auto dense, auto sparse, size_t extra_bytes, const char* name, const auto&... head) {
+        return launch_step<decltype(tpe)::value>(dense, sparse, extra_bytes, name, p, s, autoreset, st, head...,
+                                                 action_i, action_f, obs, reward, terminated, truncated, info_speed,
+                                                 info_crashed, autoreset, final_obs);
+    };
+    using hwy::highway_linear_step_kernel;
+    using hwy::highway_step_kernel;
+    if (p->n_agents <= 1)
+        return with_tpe(p->n_vehicles, [&](auto tpe) {
+            constexpr int TPE = decltype(tpe)::value;
+            const size_t linear_bytes = sizeof(hwy::LinearShared<TPE>);
+            if (al)
+                return t ? launch(tpe, highway_linear_step_kernel<TPE, true, true>,
+                                  highway_linear_step_kernel<TPE, true, false>, linear_bytes,
+                                  "highway_linear_step_kernel", *p, *s, *t)
+                         : launch(tpe, highway_step_kernel<TPE, true, true>, highway_step_kernel<TPE, true, false>, 0,
+                                  "highway_step_kernel", *p, *s);
+            return t ? launch(tpe, highway_linear_step_kernel<TPE, false, true>,
+                              highway_linear_step_kernel<TPE, false, false>, linear_bytes, "highway_linear_step_kernel",
+                              *p, *s, *t)
+                     : launch(tpe, highway_step_kernel<TPE, false, true>, highway_step_kernel<TPE, false, false>, 0,
+                              "highway_step_kernel", *p, *s);
+        });
+    if (!al)
+        return fail("%s", "several controlled vehicles need a congruent lane table (no general-geometry multi-agent "
+                          "kernel)");
+    return with_tpe(p->n_vehicles, [&](auto tpe) {
+        constexpr int TPE = decltype(tpe)::value;
+        return launch(tpe, hwy::highway_multi_step_kernel<TPE, true>, hwy::highway_multi_step_kernel<TPE, false>,
+                      sizeof(hwy::MultiShared<TPE>), "highway_multi_step_kernel", *p, *s);
+    });
 }
 }  // namespace
 

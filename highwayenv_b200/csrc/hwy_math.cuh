@@ -109,24 +109,16 @@ __device__ __forceinline__ double div_finite(double n, double d) { return n == 0
 // exp(y log x) — the error of log(x) is multiplied by y log x — is small here because |d log x| <= 0.35 for x in
 // [0.5, 2] (ratios of a speed to its target): ~1.5 ulp on top of the two functions' own 1 ulp, the same class as the
 // library pow's 2 ulp bound.  For small x the rounding of d * log(x) (|d log x| <= 69 down to x = 1e-60) dominates:
-// a relative error below 1e-14, irrelevant where (1 - x^delta) is what is used.  It replaces ~175 issued instructions per call by ~80.  HWY_LIBRARY_POW restores the library call.
+// a relative error below 1e-14, irrelevant where (1 - x^delta) is what is used.  It replaces ~175 issued instructions per call by ~80.
 static __device__ __noinline__ double m_exp_dlog(double d, double x) { return exp(d * log(x)); }
 __device__ __forceinline__ double idm_pow(double x, double delta) {
-#ifndef HWY_LIBRARY_POW
     if (x < 1e60 && fabs(delta - 4.0) <= 0.5) {
-#else
-    if (delta == 4.0 && x < 1e70) {
-#endif
         const double p = x * x, e = fma(x, x, -p);
         const double q = p * p, f = fma(p, p, -q);
         const double x4 = q + (f + 2.0 * (p * e));
-#ifndef HWY_LIBRARY_POW
         if (delta == 4.0) return x4;
         if (x > 1e-60) return x4 * m_exp_dlog(delta - 4.0, x);
         if (x == 0.0) return 0.0;  // 0 ** delta, delta > 0
-#else
-        return x4;
-#endif
     }
     return m_pow(x, delta);
 }

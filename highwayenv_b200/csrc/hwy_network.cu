@@ -17,7 +17,6 @@
 // The lane table lives in HBM (HwyNetGraph) and is staged into shared memory once per block.  DESIGN.md 3.5-3.9.
 //
 // Reference paths are relative to /root/reference/highway_env.
-#include <atomic>
 #include <cstdio>
 #include <mutex>
 
@@ -39,10 +38,7 @@ constexpr int kBlockThreads = 256;  // observe / substeps / debug kernels
 // ~110 KB of SASS against a much smaller instruction cache, and two co-resident blocks in different phases evict each
 // other: 512 x 1 was faster than 256 x 2 (same warps per SM) and 128 x 4.  The
 // launch uses fewer threads per block when that spreads the envs over all SMs (step_plan).
-#ifndef HWY_NET_STEP_THREADS
-#define HWY_NET_STEP_THREADS 512
-#endif
-constexpr int kStepThreads = HWY_NET_STEP_THREADS;
+constexpr int kStepThreads = 512;
 constexpr int kPred = 11;  // np.arange(0.25, 3, 0.25) prediction points of RegulatedRoad.is_conflict_possible
 constexpr int kPredChunk = 4;  // horizon points staged in shared memory at a time
 
@@ -397,14 +393,10 @@ __device__ __forceinline__ void group_sync() {
 // phase lets them share the fetched lines instead of each streaming the whole body (stall_no_instruction).
 template <int G>
 __device__ __forceinline__ void phase_sync() {
-#ifdef HWY_NET_WARP_PHASES
-    __syncwarp(group_mask<G>());
-#else
     // NOT __syncthreads(): that is barrier.sync.ALIGNED, which requires the whole warp to arrive converged — the
     // compiler does not guarantee that here (per-vehicle branches around the call sites; synccheck flagged it).
     // The unaligned form counts threads individually and is also the intra-group memory fence the callers need.
     asm volatile("barrier.sync 0;" ::: "memory");
-#endif
 }
 
 // road/road.py:55-71 get_closest_lane_index for every vehicle of the group; also refreshes the own-lane
@@ -896,11 +888,7 @@ __device__ __forceinline__ bool has_corner_inside(double c1x, double c1y, double
     double s1, c1, s2, c2;
     m_sincos(a1, &s1, &c1);
     m_sincos(a2, &s2, &c2);
-#ifdef HWY_NET_INLINE_RECT
-#pragma unroll
-#else
 #pragma unroll 1
-#endif
     for (int k = 0; k < 9; ++k) {
         double px = c1 * pxs[k] + (-s1) * pys[k] + c1x;
         double py = s1 * pxs[k] + c1 * pys[k] + c1y;
@@ -995,14 +983,7 @@ __device__ __forceinline__ void enforce_road_rules(const bool dynamical, const G
                 double p1x = st.pred[a][k][0], p1y = st.pred[a][k][1], p2x = st.pred[b][k][0], p2y = st.pred[b][k][1];
                 if (norm2(p2x - p1x, p2y - p1y) > kVehLength) continue;
                 double h1 = st.pred[a][k][2], h2 = st.pred[b][k][2];
-#ifdef HWY_NET_INLINE_RECT
-                hit = has_corner_inside(p1x, p1y, 1.5 * kVehLength, 0.9 * kVehWidth, h1, p2x, p2y, 1.5 * kVehLength,
-                                        0.9 * kVehWidth, h2) ||
-                      has_corner_inside(p2x, p2y, 1.5 * kVehLength, 0.9 * kVehWidth, h2, p1x, p1y, 1.5 * kVehLength,
-                                        0.9 * kVehWidth, h1);
-#else
                 hit = rotated_rectangles_intersect(p1x, p1y, h1, p2x, p2y, h2, 1.5 * kVehLength, 0.9 * kVehWidth);
-#endif
             }
             if (hit) conflict |= 1u << q;
         }
@@ -1202,17 +1183,10 @@ __device__ __forceinline__ void substep(const HwyNetParams& P, const GraphShared
     if (REG) {
         if (i == 0) st.road_steps += 1;
         group_sync<G>();
-        if (P.regulated && st.road_steps % (int)(1 / dt / 2) == 0)
-        {
-#ifdef HWY_NET_INLINE_RULES
-            if constexpr (true) {
-                enforce_road_rules<G, REG, PLAIN>(P.dynamical != 0, g, st, V, i, r, act_steer);
-            } else {
-#else
+        if (P.regulated && st.road_steps % (int)(1 / dt / 2) == 0) {
             if constexpr (PLAIN) {
                 enforce_road_rules<G, REG, true>(P.dynamical != 0, g, st, V, i, r, act_steer);
             } else {
-#endif
                 // the rules only read this vehicle's flags and speed and only move its target speed and YIELDING bit:
                 // a real call with those in registers keeps 10 KB that run every 7th substep out of the loop body
                 const int code = enforce_road_rules_call<G, REG>(g, st, V, i, r.meta, r.speed);
@@ -1294,23 +1268,8 @@ __device__ __forceinline__ void substep(const HwyNetParams& P, const GraphShared
             const int a = i < j ? i : j, b = i < j ? j : i;
             const bool b_object = st.kind[b] == HWY_KIND_OBSTACLE;
             double tr[2];
-#ifdef HWY_NET_INLINE_COLLIDE
-            int flags = 0;
-            {
-                const double len_b = b_object ? 2.0 : kVehLength;
-                const double dist = norm2(st.x[b] - st.x[a], st.y[b] - st.y[a]);
-                if (dist > (diag_v + (b_object ? diag_o : diag_v)) / 2 + st.v[a] * dt) continue;
-                Quad pa = make_polygon(st.x[a], st.y[a], st.c[a], st.s[a]);
-                Quad pb = make_polygon(st.x[b], st.y[b], st.c[b], st.s[b], len_b);
-                bool inter, will;
-                polygons_intersecting(pa, pb, st.v[a] * st.c[a] * dt, st.v[a] * st.s[a] * dt, st.v[b] * st.c[b] * dt,
-                                      st.v[b] * st.s[b] * dt, inter, will, tr[0], tr[1]);
-                flags = (will ? 1 : 0) | (inter ? 2 : 0);
-            }
-#else
             const int flags = collide_exact(st.x[a], st.y[a], st.c[a], st.s[a], st.v[a], st.x[b], st.y[b], st.c[b], st.s[b],
                                             st.v[b], b_object, dt, tr);
-#endif
             if ((flags & 1) && !(b_object && i == b)) {
                 const double share = b_object ? 1.0 : 0.5;
                 r.imp_x = i == a ? tr[0] * share : -tr[0] * share;
@@ -2638,12 +2597,7 @@ int validate_net(const HwyNetParams* p, const HwyNetGraph* graph, const HwyNetSt
         return fail("%s", "null state pointer");
     if (s->vp == HWY_NET_GROUP_LARGE && (!s->count || !s->road_steps)) return fail("%s", "count / road_steps required");
     if (p->n_agents < 0 || p->n_agents > 4) return fail("%s", "n_agents out of range (0..4)");
-    int dev_count = 0;
-    if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count < 1) {
-        cudaGetLastError();
-        return fail("%s", "no CUDA device: this library has no CPU fallback");
-    }
-    return 0;
+    return hwy_abi::require_device();
 }
 
 // one side stream (+ fork / join events) per device, created on first use
@@ -2655,10 +2609,7 @@ SideStream* side_stream() {
     static std::mutex mu;
     static SideStream* table[64] = {nullptr};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
-        fail("%s", "cudaGetDevice failed");
-        return nullptr;
-    }
+    if (hwy_abi::current_device(dev)) return nullptr;
     std::lock_guard<std::mutex> lock(mu);
     if (!table[dev]) {
         SideStream* s = new SideStream;
@@ -2679,12 +2630,6 @@ template <int G, bool REG>
 size_t stage_smem_bytes(int per) {
     return ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) + (size_t)per * sizeof(hwynet::EnvStage<G, REG>);
 }
-template <typename K>
-int configure_smem(K kernel, size_t bytes) {
-    cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-    return 0;
-}
 int blocks_for(int n_envs, int g) {
     int per = hwynet::kBlockThreads / g;
     return (n_envs + per - 1) / per;
@@ -2698,31 +2643,21 @@ struct StepPlan {
     int threads, blocks, per;
     size_t smem;
 };
-int sm_count() {
-    static std::atomic<int> cached[64];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-    int n = cached[dev].load(std::memory_order_relaxed);
-    if (n == 0) {
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
-        cached[dev].store(n, std::memory_order_relaxed);
-    }
-    return n;
-}
 template <int G, bool REG>
-StepPlan step_plan(int n_envs) {
-    const int per_max = hwynet::kStepThreads / G, sms = sm_count();
+int step_plan(int n_envs, StepPlan& plan) {
+    hwy_abi::DeviceProps d;
+    if (hwy_abi::device_props(d)) return 1;
+    const int per_max = hwynet::kStepThreads / G, sms = d.n_sm;
     const int waves = (n_envs + sms * per_max - 1) / (sms * per_max);
     int per = (n_envs + waves * sms - 1) / (waves * sms);
     int threads = ((per * G + 31) / 32) * 32;
     if (threads > hwynet::kStepThreads) threads = hwynet::kStepThreads;
     per = threads / G;
-    StepPlan plan;
     plan.threads = threads;
     plan.per = per;
     plan.blocks = (n_envs + per - 1) / per;
     plan.smem = stage_smem_bytes<G, REG>(per);
-    return plan;
+    return 0;
 }
 
 template <int G, bool REG>
@@ -2730,11 +2665,12 @@ int launch_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyInters
                 const int32_t* action, float* obs, double* reward, uint8_t* terminated, uint8_t* truncated,
                 double* info_speed, uint8_t* info_crashed, cudaStream_t st, const int* list = nullptr,
                 double* agents_reward = nullptr, uint8_t* agents_terminated = nullptr) {
-    const StepPlan plan = step_plan<G, REG>(s->n_envs);
+    StepPlan plan;
+    if (step_plan<G, REG>(s->n_envs, plan)) return 1;
     const size_t smem_max = stage_smem_bytes<G, REG>(hwynet::kStepThreads / G);
     if constexpr (REG) {
         if (p->action_type == 1) {  // a ContinuousAction ego (plain Vehicle / BicycleVehicle): its own instantiation
-            if (configure_smem(hwynet::network_step_kernel<G, REG, true>, smem_max)) return 1;
+            if (hwy_abi::opt_in_smem((const void*)hwynet::network_step_kernel<G, REG, true>, smem_max)) return 1;
             hwynet::network_step_kernel<G, REG, true><<<plan.blocks, plan.threads, plan.smem, st>>>(
                 *p, graph, *s, sp, action, obs, reward, terminated, truncated, info_speed, info_crashed, list,
                 agents_reward, agents_terminated);
@@ -2742,7 +2678,7 @@ int launch_step(const HwyNetParams* p, const HwyNetGraph* graph, const HwyInters
         }
     }
     if (p->action_type == 1) return fail("%s", "ContinuousAction is implemented on the intersection family (32-slot state)");
-    if (configure_smem(hwynet::network_step_kernel<G, REG, false>, smem_max)) return 1;
+    if (hwy_abi::opt_in_smem((const void*)hwynet::network_step_kernel<G, REG, false>, smem_max)) return 1;
     hwynet::network_step_kernel<G, REG, false><<<plan.blocks, plan.threads, plan.smem, st>>>(
         *p, graph, *s, sp, action, obs, reward, terminated, truncated, info_speed, info_crashed, list, agents_reward,
         agents_terminated);
@@ -2763,7 +2699,7 @@ int launch_groups(KernelFor kernel_for, const char* name, const HwyNetState* s, 
         using T = decltype(slots);
         const auto kernel = kernel_for(slots);
         const size_t smem = stage_smem_bytes<T::G, T::REG>(hwynet::kBlockThreads / T::G);
-        if (configure_smem(kernel, smem)) return 1;
+        if (hwy_abi::opt_in_smem((const void*)kernel, smem)) return 1;
         kernel<<<blocks_for(s->n_envs, T::G), hwynet::kBlockThreads, smem, st>>>(args...);
         return check_launch(name);
     };
@@ -2784,7 +2720,7 @@ int launch_intersection_reset(const HwyNetParams* p, const HwyNetGraph* graph, c
                               const HwyNetState* s, float* obs, cudaStream_t st) {
     constexpr int kThreads = 64, per = kThreads / G;
     const size_t smem = stage_smem_bytes<G, true>(per);
-    if (configure_smem(hwynet::intersection_reset_kernel<G, true>, smem)) return 1;
+    if (hwy_abi::opt_in_smem((const void*)hwynet::intersection_reset_kernel<G, true>, smem)) return 1;
     hwynet::intersection_reset_kernel<G, true>
         <<<(s->n_envs + per - 1) / per, kThreads, smem, st>>>(*p, graph, *s, *spawn, spawn->scratch, obs);
     return check_launch("intersection_reset_kernel");
@@ -2842,8 +2778,11 @@ int launch_racetrack(const HwyNetParams* p, const HwyNetGraph* graph, const HwyR
                      uint8_t* terminated, uint8_t* truncated, double* info_speed, uint8_t* info_crashed,
                      cudaStream_t st) {
     constexpr int G = HWY_NET_GROUP;
-    const StepPlan plan = step_plan<G, false>(s->n_envs);
-    if (configure_smem(hwynet::racetrack_step_kernel<G>, stage_smem_bytes<G, false>(hwynet::kStepThreads / G))) return 1;
+    StepPlan plan;
+    if (step_plan<G, false>(s->n_envs, plan)) return 1;
+    if (hwy_abi::opt_in_smem((const void*)hwynet::racetrack_step_kernel<G>,
+                             stage_smem_bytes<G, false>(hwynet::kStepThreads / G)))
+        return 1;
     hwynet::racetrack_step_kernel<G><<<plan.blocks, plan.threads, plan.smem, st>>>(
         *p, graph, rp, *s, action, n_substeps, obs, reward, terminated, truncated, info_speed, info_crashed);
     return check_launch("racetrack_step_kernel");

@@ -516,12 +516,7 @@ int validate_view(const HwyObsView* v) {
     if (!v->pos || !v->hs || !v->meta) return fail("%s", "null state pointer in view");
     if (!v->count && (v->n_vehicles < 1 || v->n_vehicles > v->vp)) return fail("%s", "n_vehicles out of range");
     if (v->n_agents < 0 || v->n_agents > 8) return fail("%s", "n_agents out of range");
-    int dev_count = 0;
-    if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count < 1) {
-        cudaGetLastError();
-        return fail("%s", "no CUDA device: this library has no CPU fallback");
-    }
-    return 0;
+    return hwy_abi::require_device();
 }
 int agents_of(const HwyObsView* v) { return v->n_agents > 1 ? v->n_agents : 1; }
 }  // namespace
@@ -540,8 +535,7 @@ int hwy_observe_grid(const HwyNetGraph* graph, const HwyObsView* view, const Hwy
     const size_t smem = ((sizeof(hwynet::GraphShared) + 15) & ~size_t(15)) + (size_t)cells * 5 + 16;
     if (smem > 200 * 1024) return fail("%s", "OccupancyGrid too large for one block's shared memory (cells <= ~38000)");
     if (!(p->grid_step[0] > 0) || !(p->grid_step[1] > 0)) return fail("%s", "grid_step must be positive");
-    cudaError_t err = cudaFuncSetAttribute(hwyobs::grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
+    if (hwy_abi::opt_in_smem((const void*)hwyobs::grid_kernel, smem)) return 1;
     hwyobs::grid_kernel<<<view->n_envs * agents_of(view), hwyobs::kThreads, smem, (cudaStream_t)stream>>>(
         graph, *view, *p, mask_a, mask_b, obs);
     return check_launch("observe grid_kernel");

@@ -436,22 +436,11 @@ extern "C" int hwy_value_iteration(const HwyValueIterationParams* p, const int32
     if (p->iterations < 0) return fail("%s", "iterations must be >= 0");
     if (!(p->gamma >= 0.0 && p->gamma <= 1.0)) return fail("%s", "gamma must be in [0, 1]");
     if ((p->state == nullptr) != (p->action == nullptr)) return fail("%s", "state and action go together");
-    int dev_count = 0;
-    if (cudaGetDeviceCount(&dev_count) != cudaSuccess || dev_count < 1) {
-        cudaGetLastError();
-        return fail("%s", "no CUDA device: this library has no CPU fallback");
-    }
-    // the opt-in to the largest size is made once (a later call may be under CUDA-graph capture); every launch passes
-    // its own 3 * s_max doubles.  Per device.
-    static bool opted_in[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fail("%s", "cudaGetDevice failed");
-    if (!opted_in[dev]) {
-        cudaError_t err = cudaFuncSetAttribute(hwyplan::value_iteration_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               3 * HWY_VI_MAX_STATES * (int)sizeof(double));
-        if (err != cudaSuccess) return fail("cudaFuncSetAttribute: %s", cudaGetErrorString(err));
-        opted_in[dev] = true;
-    }
+    if (hwy_abi::require_device()) return 1;
+    // The opt-in is to the largest size, made by the first call on a device, so that no later call has to raise it (a
+    // later call may be under CUDA-graph capture); every launch passes its own 3 * s_max doubles.
+    if (hwy_abi::opt_in_smem((const void*)hwyplan::value_iteration_kernel, 3 * HWY_VI_MAX_STATES * sizeof(double)))
+        return 1;
     const int smem = 3 * p->s_max * (int)sizeof(double);
     hwyplan::value_iteration_kernel<<<p->n_envs, hwyplan::kThreads, smem, (cudaStream_t)stream>>>(
         *p, transition, reward, terminal, n_states, q, iterations_done);
